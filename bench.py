@@ -16,8 +16,10 @@ One "step" = one pass of the chain over the rank's frames:
           H2D and D2H copies inside the timed region; e2e.stock_nodes = the same chain as four unchanged ComfyUI nodes
   extra : configs[1] (64 x 1080p fp16, grain + LUT + unsharp), "grain + LUT + unsharp at 4K fp32", configs[2] (colour match alone: LAB
           transfer and histogram mode, reference statistics gathered every step), configs[4] (temporal sharpen), each with its own roofline
-  --impl reference : the reference's CPU path for the same chain (oracle port of the reference nodes; /root/reference
-          does not exist on the GPU box) on all host cores, rank 0 only, bounded sample per step
+  --impl reference : the reference's CPU path for the same chain (oracle port of the reference nodes) on all host cores,
+          rank 0 only, 2 frames per step
+  --dump-outputs DIR : after the timed steps, what the timed path computed in its last step as DIR/<name>.npy (a fixed sample of
+          the frames; for the headline chain also its reference statistics)
 """
 import argparse
 import importlib
@@ -34,8 +36,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):
 
 
 def host_threads():
-    """Threads for the CPU arm: one per PHYSICAL core (torch's own default; measured on the GPU box: 128 SMT threads run the
-    reference chain 3x slower than 64)."""
+    """Threads for the CPU arm: one per PHYSICAL core (torch's own default; SMT siblings slow the reference chain down)."""
     try:
         import psutil
         n = psutil.cpu_count(logical=False)
@@ -68,24 +69,7 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def recorded_traffic(key):
-    """dram bytes per launch of a kernel from the committed ncu capture (profiles/dominant_kernel.json), with a staleness flag:
-    the capture is only valid for the kernel sources it was taken from (content hash of csrc/ + the header)."""
-    path = os.path.join(ROOT, "profiles", "dominant_kernel.json")
-    if not os.path.exists(path):
-        return None, None
-    with open(path) as fh:
-        d = json.load(fh).get(key)
-    if not d:
-        return None, None
-    try:
-        cur = importlib.import_module(PKG + ".build")._source_hash()
-    except Exception:
-        cur = None
-    return d.get("dram_bytes_per_launch"), {"capture": d.get("capture"), "traffic_stale": bool(cur is None or d.get("src_hash") != cur)}
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler(threading.Thread):
@@ -150,6 +134,24 @@ def device_natural_frames(n, h, w, seed, dtype, dev):
     return (acc * gain + off).clamp_(0, 1).permute(0, 2, 3, 1).contiguous().to(dtype)
 
 
+DUMP_PIXELS = 1 << 21          # pixels in the dumped sample over all ranks: 2 Mi x 3 fp32 = 24 MiB
+
+
+def dump_outputs(path, out, ref_sums=None, rank=None, world=1):
+    """What the timed step handed its caller in the last step, as .npy files under `path`: the reference statistics (float64, whole;
+    the headline chain only) and a fixed sample of the output frames (float32, DUMP_PIXELS / world pixels per rank at indices drawn
+    from a CPU generator with a fixed seed, so that two builds given the same arguments dump the same pixels).  The full output
+    (12.7 GB at 128 frames) would not fit the 64 MB budget."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    tag = "" if rank is None else "_rank%d" % rank
+    flat = out.reshape(-1, out.shape[-1])
+    idx = torch.randint(0, flat.shape[0], (min(DUMP_PIXELS // world, flat.shape[0]),), generator=torch.Generator().manual_seed(20240601))
+    np.save(os.path.join(path, "frames_out_sample%s.npy" % tag), flat[idx.to(out.device)].float().cpu().numpy())
+    if ref_sums is not None:
+        np.save(os.path.join(path, "reference_sums%s.npy" % tag), ref_sums.double().cpu().numpy())
+
+
 def tile_frames(base, total):
     """`total` frames from the distinct `base` frames (repeated; a per-frame offset keeps every frame's statistics distinct)"""
     n = base.shape[0]
@@ -197,21 +199,25 @@ def run_reference(args):
     lut = oracle.parse_cube(LUT_FILE)
 
     def step():
+        torch.manual_seed(123)                                 # the grain's torch.randn draw: identical inputs from run to run
         a = oracle.film_grain(x, GRAIN["intensity"], GRAIN["saturation_mix"], batch_size=4)
         b = oracle.color_match(a, ref, 1.0, 1)
         c = oracle.apply_lut(b, lut, 10.0)
         return oracle.unsharp_numpy(c, SHARPEN)
-    step()
-    steps = max(1, min(args.steps, 3))
+    for _ in range(args.warmup):
+        step()
+    steps = args.steps
     t0 = time.perf_counter()
     for _ in range(steps):
-        step()
+        res = step()
     dt = (time.perf_counter() - t0) / steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, res)
     mps = sample_frames * H4K * W4K / 1e6 / dt
     sample = ("%d x 3840x2160 fp32 frames per step through the reference CPU nodes FastFilmGrain -> ColorMatchToReference -> VRGDG_LUTS -> "
               "FastUnsharpSharpen (numpy path), oracle port" % sample_frames)
     print(json.dumps({
-        "impl": "reference", "metric": METRIC, "value": round(mps, 3), "unit": "MP/s", "n_gpus": args.gpus, "steps": steps, "warmup": 1,
+        "impl": "reference", "metric": METRIC, "value": round(mps, 3), "unit": "MP/s", "n_gpus": args.gpus, "steps": steps, "warmup": args.warmup,
         "ms_per_step": round(dt * 1e3, 2), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "sample": sample},
         "cpu_baseline": {"value": round(mps, 3), "unit": "MP/s", "cores": threads, "kind": "port", "sample": sample},
@@ -220,7 +226,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------------------------------
-# B200 arm
+# CUDA arm
 # ------------------------------------------------------------------------------------------------------------------------
 def run_b200(args):
     rank, world, local = dist_env()
@@ -290,6 +296,8 @@ def run_b200(args):
     sampler.start()
     ms_step, launches = timed(step, args.steps, 0)
     sampler.stop_flag.set()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out, chain._ref_sums, rank if world > 1 else None, world)   # before the other legs overwrite `out`
     value = world * npix / 1e6 / (ms_step / 1e3)
     tile_path = nv.last_tile_path()
     ref_sums_identical = True
@@ -339,11 +347,10 @@ def run_b200(args):
         o2 = torch.empty_like(x2)
         ms2, _ = timed(lambda: c4(x2, first_frame=rank * 64, out=o2), ex_steps, 3)
         n2 = 64 * 1080 * 1920
-        tr2, st2 = recorded_traffic("configs1_f16")
         extras["configs1_grain_lut_unsharp_1080p_f16"] = {
             "workload": "configs[1]: fused grain + 33^3 LUT + unsharp, 64 x 1920x1080 fp16 frames per GPU, one k_tile launch per step",
             "value": round(world * n2 / 1e6 / (ms2 / 1e3), 1), "unit": "MP/s", "ms_per_step": round(ms2, 4), "steps": ex_steps,
-            "roofline": roofline(n2 * 12, ms2, dict({"kernel": "k_tile<half, grain|lut>", "traffic": tr2}, **(st2 or {})))}
+            "roofline": roofline(n2 * 12, ms2, {"kernel": "k_tile<half, grain|lut>"})}
         del x2, o2, c4
         # configs[2]: colour match alone on 4K fp32 frames (256 frames over 8 GPUs = 32 per GPU) against one reference frame, the reference
         # statistics gathered over NCCL inside every step: (a) the reference's algorithm (LAB mean / std transfer, nodes.py:91-124),
@@ -393,7 +400,7 @@ def run_b200(args):
     host_in.copy_(x[:nE])
     host_out = torch.empty_like(host_in, pin_memory=True)      # pinned once, reused every step
     e2e_steps = max(1, min(args.steps, 5))
-    chunk = int(os.environ.get("VRGDG_BENCH_CHUNK", "1"))       # measured: 1 frame per chunk 3838 MP/s, 2 frames 3690 (shorter pipeline fill / drain)
+    chunk = int(os.environ.get("VRGDG_BENCH_CHUNK", "1"))       # one frame per chunk: shortest pipeline fill / drain
 
     def e2e_step():
         chain.set_reference(ref_sums=vdist.reference_sums_distributed(ref))
@@ -449,7 +456,6 @@ def run_b200(args):
 
     if rank == 0:
         alg = npix * 24                                       # 12 B read + 12 B written per fp32 pixel, SURVEY 8(d)
-        tr, st = recorded_traffic("headline_apply")
         line = {
             "metric": METRIC, "value": round(value, 1), "unit": "MP/s", "n_gpus": world, "steps": args.steps, "warmup": warm,
             "ms_per_step": round(ms_step, 4), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
@@ -459,18 +465,15 @@ def run_b200(args):
                        "parallelism": "frame-sharded dp%d; colour-match reference rows sharded, one 56-byte all-gather per step" % world,
                        "collective": ("nccl all_gather inside every step" if world > 1 else "none at N=1 (single rank computes the whole reference frame)"),
                        "ref_sums_identical_on_all_ranks": ref_sums_identical,
-                       "l2": "input (12.7 GB per GPU) and output are each far larger than L2 (126 MB); no flush needed", "tile_path": tile_path,
+                       "l2": "input (12.7 GB per GPU) and output are each far larger than L2 (50 MB); no flush needed", "tile_path": tile_path,
                        "numa_bound_cpus": len(numa_cpus) if numa_cpus else None},
-            "roofline": dict(roofline(alg, ms_step, {
+            "roofline": roofline(alg, ms_step, {
                 "kernel": "the whole step: k_lab_moments<float, grain, store f-planes> + k_moments_final + k_colormatch_params + "
-                          "k_tile<float, colormatch-from-f | lut, unsharp>, 16 groups of 8 frames (vrgdg_chain_cm_apply); "
-                          "per-kernel shares: profiles/ launch list",
+                          "k_tile<float, colormatch-from-f | lut, unsharp>, 16 groups of 8 frames (vrgdg_chain_cm_apply)",
                 "moved_bytes_per_pixel": 48, "algorithmic_bytes_per_pixel": 24,
                 "limiter": "not HBM: the statistics pass is bound by instruction issue / the XU (MUFU) pipe (Philox + Box-Muller, six fractional "
-                           "powers per pixel), the apply pass by the L1 data pipe (three 32-byte lane accesses per pixel for the LUT cell, 83 % busy); "
-                           "the two passes of neighbouring frame groups run concurrently (pipelined schedule); HBM carries 48 B/px at ~0.4 of its "
-                           "peak: see profiles/README.md",
-                "traffic": tr}), **(st or {})),
+                           "powers per pixel), the apply pass by the L1 data pipe (three 32-byte lane accesses per pixel for the LUT cell); "
+                           "the two passes of neighbouring frame groups run concurrently (pipelined schedule); HBM carries 48 B/px"}),
             "schedules_ms_per_step": dict({"f_planes_pipelined_one_call (headline)": round(ms_step, 4)}, **alt),
             "e2e": {"value": round(e2e_value, 1), "unit": "MP/s", "h2d_bytes_per_step": e2e_bytes, "d2h_bytes_per_step": e2e_bytes,
                     "ms_per_step": round(e2e_ms, 3), "steps": e2e_steps, "frames_per_gpu": nE,
@@ -499,7 +502,11 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra lines and the stock-node leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the headline step computed in its last step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-"""comfyui-vrgamedevgirl_b200 — B200-native (sm_100a) implementation of the per-pixel video post-processing
+"""comfyui-vrgamedevgirl_b200 — H100-native (sm_90a) implementation of the per-pixel video post-processing
 hot path of the comfyui-vrgamedevgirl node pack, behind the same ComfyUI node API.
 
 ComfyUI loads this directory as a custom node package and reads NODE_CLASS_MAPPINGS /

@@ -1,7 +1,7 @@
 """ctypes binding of libvrgdg_b200.so (C ABI: include/vrgdg_b200.h).
 
 There is deliberately no fallback: if the library is missing, was built for another architecture, or no
-CUDA device is visible, every operation raises.  The filters exist only as sm_100a kernels.
+CUDA device is visible, every operation raises.  The filters exist only as sm_90a kernels.
 """
 import ctypes
 import os

@@ -21,7 +21,7 @@ def compute_device(hint=None):
         if dev.type == "cuda":
             return dev
     if not torch.cuda.is_available():
-        raise RuntimeError("vrgdg_b200: no CUDA device is available; these nodes are sm_100a kernels and have no CPU path")
+        raise RuntimeError("vrgdg_b200: no CUDA device is available; these nodes are sm_90a kernels and have no CPU path")
     return torch.device("cuda", torch.cuda.current_device())
 
 

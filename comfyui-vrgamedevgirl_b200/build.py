@@ -1,4 +1,4 @@
-"""Build libvrgdg_b200.so (sm_100a only) in-tree with nvcc.  No GPU is needed to build.
+"""Build libvrgdg_b200.so (sm_90a only) in-tree with nvcc.  No GPU is needed to build.
 
     python comfyui-vrgamedevgirl_b200/build.py [--force]
 
@@ -19,8 +19,9 @@ LIB = os.path.join(LIBDIR, "libvrgdg_b200.so")
 STAMP = LIB + ".srchash"
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 UNITS = ["vrgdg_abi.cu", "vrgdg_f32.cu", "vrgdg_f16.cu", "vrgdg_bf16.cu", "vrgdg_u8.cu"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
+    "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-Xfatbin", "-compress-all", "-I", INCLUDE,
 ]
 
@@ -78,7 +79,7 @@ def build(force=False, verbose=True):
 
     with ThreadPoolExecutor(max_workers=len(UNITS)) as ex:
         objs = list(ex.map(compile_one, UNITS))
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-lcudart_static", "-lpthread", "-ldl", "-lrt"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-Xcompiler", "-fPIC", "-lcudart_static", "-lpthread", "-ldl", "-lrt"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -51,7 +51,7 @@ class VRGDG_B200_PostChain:
     RETURN_TYPES = ("IMAGE",)
     FUNCTION = "apply_chain"
     CATEGORY = "video/enhancement"
-    DESCRIPTION = "Film grain, colour match, 3D LUT and sharpen fused into one GPU pass (B200)."
+    DESCRIPTION = "Film grain, colour match, 3D LUT and sharpen fused into one GPU pass (H100)."
 
     def apply_chain(self, images, grain_intensity, saturation_mix, match_strength, lut_name, lut_strength, sharpen, sharpen_strength, use_gpu,
                     batch_size, reference_image=None):
@@ -139,7 +139,7 @@ class VRGDG_B200_HistogramColorMatch:
     RETURN_TYPES = ("IMAGE",)
     FUNCTION = "match_histogram"
     CATEGORY = "video/enhancement"
-    DESCRIPTION = "Matches each frame's per-channel histogram to a reference image (monotone CDF transfer, B200)."
+    DESCRIPTION = "Matches each frame's per-channel histogram to a reference image (monotone CDF transfer, H100)."
 
     def match_histogram(self, images, reference_image, match_strength, batch_size):
         from . import ops
@@ -175,7 +175,7 @@ class VRGDG_B200_TemporalSharpen:
     RETURN_TYPES = ("IMAGE",)
     FUNCTION = "sharpen"
     CATEGORY = "video/enhancement"
-    DESCRIPTION = "Temporal unsharp mask: each frame is sharpened against the mean of itself and its two neighbours (B200)."
+    DESCRIPTION = "Temporal unsharp mask: each frame is sharpened against the mean of itself and its two neighbours (H100)."
 
     def sharpen(self, images, strength, batch_size):
         from . import ops

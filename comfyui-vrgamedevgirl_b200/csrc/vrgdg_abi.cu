@@ -44,15 +44,17 @@ int get_ctx(void* stream, LaunchCtx& ctx) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return fail_cuda(e, "cudaGetDevice");
-  static thread_local int cached_dev = -1, cached_sms = 0, cached_major = 0;
+  static thread_local int cached_dev = -1, cached_sms = 0, cached_major = 0, cached_minor = 0;
   if (cached_dev != dev) {
-    int sms = 0, major = 0;
+    int sms = 0, major = 0, minor = 0;
     if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
     if ((e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
-    cached_dev = dev; cached_sms = sms; cached_major = major;
+    if ((e = cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
+    cached_dev = dev; cached_sms = sms; cached_major = major; cached_minor = minor;
   }
-  if (cached_major != 10)
-    return fail(VRGDG_E_UNSUPPORTED, "libvrgdg_b200 holds sm_100a code only; device %d has compute capability major %d", dev, cached_major);
+  if (cached_major != 9 || cached_minor != 0)   // sm_90a code runs on compute capability 9.0 only
+    return fail(VRGDG_E_UNSUPPORTED, "libvrgdg_b200 holds sm_90a code only; device %d has compute capability %d.%d", dev, cached_major,
+                cached_minor);
   ctx.stream = reinterpret_cast<cudaStream_t>(stream);
   ctx.sms = cached_sms;
   return VRGDG_OK;
@@ -492,8 +494,8 @@ int vrgdg_chain_lab_moments_ext(const void* in, int B, int H, int W, int dtype, 
 static int cm_group_frames(int B, int H, int W, int dtype, int flags, int group_frames) {
   (void)dtype; (void)flags;
   if (group_frames > 0) return group_frames < B ? group_frames : (B > 0 ? B : 1);
-  // Measured (profiles/README.md, round 2): both passes are instruction-issue bound, so keeping a group's re-read set inside L2
-  // (1-2 frames per group) buys nothing, while short launches lose 5-20 % to their last partial wave of tiles.  Default = about
+  // Both passes are instruction-issue bound, so keeping a group's re-read set inside L2 (1-2 frames per group) buys nothing, while
+  // short launches lose to their last partial wave of tiles.  Default = about
   // 64 Mpixel per group (8 x 4K, 32 x 1080p): > 25 000 tiles per launch, <= 800 MB of f-planes per buffer.
   const int64_t px = (int64_t)H * W;
   int64_t g = px > 0 ? (((int64_t)64 << 20) + px - 1) / px : 1;
@@ -566,7 +568,6 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
   const int NB = cm_buffers(B, G, dtype, flags);
   // statistics pass of group g+1 beside the apply pass of group g: pays when the apply pass waits on the L1 data pipe (LUT gather) and
   // leaves issue slots free; a colour match without a LUT is instruction bound in BOTH passes and runs them one after the other
-  // (measured, 32 x 4K fp32: 100 GPx/s side by side with 128-thread statistics blocks, 113 in sequence with 256-thread ones)
   const bool piped = planes && NB == 2 && desc->lut_enabled;
   char* sp = reinterpret_cast<char*>(scratch);
   double* sums = reinterpret_cast<double*>(sp);
@@ -590,7 +591,7 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
   // SM that leave exactly that much of the register file) of group g runs on a high-priority one; f-planes and partials are double
   // buffered; events fork the side streams from the caller's stream and join them back, so the call stays stream-ordered.
   // Tile CTAs of the apply pass while a statistics pass runs beside it: every tile CTA less frees registers for 3.5 more 128-thread
-  // statistics blocks.  Default from the sweep in profiles/README.md; VRGDG_PIPE_TILE_CTAS overrides (tuning only).
+  // statistics blocks.  Default 0 = no limit; VRGDG_PIPE_TILE_CTAS overrides (tuning only).
   int tile_ctas = 0;
   if (piped) {
     const char* ev = getenv("VRGDG_PIPE_TILE_CTAS");

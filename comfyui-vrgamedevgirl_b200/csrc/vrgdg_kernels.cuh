@@ -1,4 +1,4 @@
-// vrgdg_kernels.cuh — sm_100a kernels of the post-processing hot path.
+// vrgdg_kernels.cuh — sm_90a kernels of the post-processing hot path.
 //
 // Two kernel families cover every entry point of include/vrgdg_b200.h:
 //   k_point : streaming per-pixel chain  [grain][colour match][3D LUT]          (no neighbourhood)
@@ -329,9 +329,9 @@ struct TileParams {
   int grid_limit;               // > 0: launch at most this many persistent CTAs (pipelined colour-match schedule leaves room for the statistics pass)
 };
 
-// HEAVY = the LUT gather runs in the pre-stage.  Measured on the fused grain + LUT + unsharp chain (fp16 1080p, profiles/README.md):
-// one 480-thread CTA per SM 56.8 GPx/s, two 256-thread CTAs per SM 65.3-66.1 (while one CTA runs its stencil phase the other keeps
-// the L1 gather busy), three CTAs 58 (registers), 64-row tiles 65 but no room for a second CTA.  Two CTAs with a single staged
+// HEAVY = the LUT gather runs in the pre-stage.  Two 256-thread CTAs per SM beat one 480-thread CTA on the fused grain + LUT + unsharp
+// chain (while one CTA runs its stencil phase the other keeps the L1 gather busy); a third CTA runs out of registers, and 64-row tiles
+// leave no room for a second CTA.  Two CTAs with a single staged
 // tile each (the stage is refilled while the stencil runs, see EARLY in k_tile) leave ~120 KB of the SM's 228 KB as L1 for the table.
 // Everything else uses 256-thread CTAs, a 3-stage ring and 2 CTAs per SM.
 // WORK = 16-bit frames with pre-stages: their fp32 results live in a separate work tile, and a thread then produces
@@ -357,9 +357,9 @@ template <typename T, int MASK> struct TileCfg {
   // Register budget of the LUT configurations on fp32 frames: declaring a larger block than is ever launched lowers ptxas' register
   // cap (65536 / (LB_THREADS * MINB)) below the 128 that two 256-thread CTAs would allow, which leaves room in the register file for
   // the statistics blocks of the NEXT frame group next to two resident tile CTAs (pipelined colour-match schedule, vrgdg_abi.cu).
-  // Measured on the headline chain (64 x 4K fp32, profiles/r02_s2/pipe_sweep.jsonl): 256 (104-109 registers, one 128-thread statistics
-  // block fits beside two tile CTAs) 51.5 GPx/s, 320 (91-94 registers, two blocks) 55.0, 352 (80 registers + 20 bytes of spills, three
-  // blocks) 56.1; the tile kernel alone loses 0.6 % (fused grain + LUT + unsharp) to 3.7 % (serial colour-match chain) at 80 registers.
+  // 256 (104-109 registers) fits one 128-thread statistics block beside two tile CTAs, 320 (91-94 registers) two, 352 (80 registers)
+  // three or four.  At 80 registers the sm_90a LUT tile kernels spill 12-168 bytes per thread (ptxas -v).  352 was chosen by a sweep
+  // on an earlier GPU with the same register file and shared memory per SM and has not been re-swept on H100.
 #ifndef VRGDG_HEAVY_LB
 #define VRGDG_HEAVY_LB 352
 #endif
@@ -377,7 +377,7 @@ template <typename T, int MASK> struct TileCfg {
 #define VRGDG_LIGHT_NS 3
 #endif
   // plain stencils on 16-bit frames need few registers and 17 KB per staged tile: four CTAs per SM with a 2-stage ring
-  // (measured 395 -> 422 GPx/s on 1080p fp16; fp32 tiles are 35 KB per stage and gain nothing from a third CTA)
+  // (fp32 tiles are 35 KB per stage and gain nothing from a third CTA)
   static constexpr bool SLIM = (MASK == 0) && (sizeof(T) == 2);
   static constexpr int MINB = HEAVY ? VRGDG_HEAVY_MINB : (SLIM ? 4 : VRGDG_LIGHT_MINB);
   static constexpr int COLS = TXE / VEC;              // threads across
@@ -854,7 +854,7 @@ __device__ __forceinline__ void moments_add(float& r, float& g, float& b, float*
 // vrgdg_chain_cm_apply's pipelined schedule).
 #ifndef VRGDG_MOMENT_SMALL_MINB
 #define VRGDG_MOMENT_SMALL_MINB 10     // 128-thread blocks per SM the register cap is computed for: 8 = 64 registers (three blocks fit beside two
-                                       // 80-register tile CTAs), 10 = 48 registers + 12 bytes of spills (four blocks): 54.2 -> 55.5 GPx/s on the headline chain
+                                       // 80-register tile CTAs), 10 = 48 registers (four blocks; no spills on sm_90a; chosen on an earlier GPU, not re-swept on H100)
 #endif
 template <int NT> struct MomentLaunch { static constexpr int MINB = (NT == MOMENT_UNIT) ? VRGDG_MOMENT_SMALL_MINB : 4; };   // 256 threads: 64 registers as before
 template <typename T, bool GRAIN, bool VEC, int NT>

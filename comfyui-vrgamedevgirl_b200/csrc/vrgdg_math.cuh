@@ -223,9 +223,9 @@ VRGDG_HD void grain_blend_fast(float& r, float& g, float& b, float zr, float zg,
 // ---- 3D LUT trilinear: VRGDG_IV_Adjustments.py:293-336 ------------------------------------------
 // Device table layout ("cell table", built by lut_pack_entry / vrgdg_lut3d_pack): one 96-byte entry per cell origin
 //   entry (b,g,r) = rgb x { c000 c100 c010 c110 c001 c101 c011 c111 },  cXYZ = lut[min(b+Z,S-1), min(g+Y,S-1), min(r+X,S-1), :]
-// (channel-planar: one 32-byte sector per output channel) so a pixel fetches its 8 corners (24 floats) with THREE 256-bit
-// loads (LDG.E.256) from consecutive addresses instead of 24 scalar loads - or three lanes fetch one sector each.  The gather is bound by L1 tag lookups per divergent lane, not by bytes (profiles/: 4 lookups/px with a
-// 32-byte r-pair table = 60-65 Gpx/s on grained frames, 3 lookups/px with this layout = 73-84 Gpx/s, 24 scalar = 34).
+// (channel-planar: one 32-byte sector per output channel) so a pixel fetches its 8 corners (24 floats) from THREE sectors at
+// consecutive addresses (lut_load8) instead of 24 scalar loads - or three lanes fetch one sector each.  The gather is bound by L1 tag
+// lookups per divergent lane, not by bytes: 3 sectors per pixel beat both a 32-byte r-pair table (4 per pixel) and scalar loads.
 struct LutParams {
   const float* lut;      // cell table, S*S*S*24 floats: per cell three 32-byte sectors (R, G, B), 8 corners each
   const float* lutp;     // polynomial cell table (fast arithmetic only, see lutp_* below), same shape as `lut`
@@ -240,12 +240,15 @@ constexpr int LUT_CELL_FLOATS = 24;
 
 struct F8 { float v[8]; };
 
+// One 32-byte sector as two 128-bit non-coherent loads (LDG.E.128.CONSTANT): sm_90 has no 256-bit load, and both halves hit
+// the same sector, so the L2 -> L1 traffic per corner set is unchanged.
 VRGDG_HD F8 lut_load8(const float* p) {
   F8 q;
 #if defined(__CUDA_ARCH__)
-  asm("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-      : "=f"(q.v[0]), "=f"(q.v[1]), "=f"(q.v[2]), "=f"(q.v[3]), "=f"(q.v[4]), "=f"(q.v[5]), "=f"(q.v[6]), "=f"(q.v[7])
-      : "l"(p));
+  asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];"
+      : "=f"(q.v[0]), "=f"(q.v[1]), "=f"(q.v[2]), "=f"(q.v[3]) : "l"(p));
+  asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+16];"
+      : "=f"(q.v[4]), "=f"(q.v[5]), "=f"(q.v[6]), "=f"(q.v[7]) : "l"(p));
 #else
   for (int i = 0; i < 8; ++i) q.v[i] = p[i];
 #endif
@@ -312,7 +315,7 @@ VRGDG_HD void lut3d_eval(const LutParams& P, float& r, float& g, float& b) {
 
 // One output channel only: the element-mapped gather of the tile kernels (three lanes of a pixel read the three sectors of
 // one cell, i.e. one or two 128-byte lines per PIXEL instead of three per pixel: the L1 data pipe counts wavefronts per
-// distinct line and instruction; measured 73 -> 108 Gpx/s on grained frames, tools/lut_bench.cu v10 vs v13).
+// distinct line and instruction; tools/lut_bench.cu compares the two mappings as v10 and v13).
 template <bool EXACT>
 VRGDG_HD float lut3d_eval_channel(const LutParams& P, float r, float g, float b, int ch) {
   int r0, r1, g0, g1, b0, b1;
@@ -325,8 +328,8 @@ VRGDG_HD float lut3d_eval_channel(const LutParams& P, float r, float g, float b,
   return lut_channel<EXACT>(q, fr, fg, fb, subx(1.0f, fr), subx(1.0f, fg), subx(1.0f, fb));
 }
 
-// Two pixels at once: both address computations first, then all six 256-bit loads, then the lerps, so that the two
-// gathers overlap (the tile pre-stage is latency-bound on these loads: profiles/r01_v2 chain_f16_v3, two stall points).
+// Two pixels at once: both address computations first, then all six sector loads, then the lerps, so that the two
+// gathers overlap (the tile pre-stage is latency-bound on these loads).
 struct LutCell { const float* p; float fr, fg, fb; };
 
 VRGDG_HD LutCell lut_locate(const LutParams& P, float r, float g, float b) {
@@ -364,7 +367,7 @@ VRGDG_HD void lut3d_eval2(const LutParams& P, float* a, float* b) {
 //   k_000 = c000, k_100 = c100 - c000, k_010 = c010 - c000, k_110 = c110 - c100 - c010 + c000, ...  (differences along r, g, b)
 // evaluated as a nested Horner form with 7 FMAs per channel (the corner form needs 7 lerps = 14 instructions):
 //   v = (k000 + fb k001 + fg (k010 + fb k011)) + fr (k100 + fb k101 + fg (k110 + fb k111)).
-// Same 96-byte channel-planar cell, coefficient k_XYZ in the slot of corner cXYZ; three 256-bit loads per pixel as before.
+// Same 96-byte channel-planar cell, coefficient k_XYZ in the slot of corner cXYZ; three sector loads per pixel as before.
 // The coefficients are formed in double from the fp32 corners and rounded once; cell index and fractions are the exact path's.
 // Difference to the exact interpolation: a few 1e-8 of the table values (rounding of coefficients and FMAs).
 VRGDG_HD void lutp_pack_entry(const float* lut3, int S, int b, int g, int r, float* dst24) {

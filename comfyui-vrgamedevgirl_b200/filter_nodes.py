@@ -1,4 +1,4 @@
-"""The five per-pixel filter nodes of the reference's nodes.py (:18-384) on sm_100a kernels.
+"""The five per-pixel filter nodes of the reference's nodes.py (:18-384) on sm_90a kernels.
 
 Node keys, INPUT_TYPES (widget order, defaults, ranges), RETURN_TYPES, FUNCTION names, CATEGORY and method
 signatures are the reference's, so saved workflows load unchanged.  The arithmetic runs in libvrgdg_b200.so;

@@ -1,4 +1,4 @@
-"""VRGDG_LUTS / VRGDG_MakeLUT (reference: VRGDG_IV_Adjustments.py) with the trilinear sampler on sm_100a.
+"""VRGDG_LUTS / VRGDG_MakeLUT (reference: VRGDG_IV_Adjustments.py) with the trilinear sampler on sm_90a.
 
 Host-side pieces (.cube text parsing, palette-LUT construction, file naming, cache keys) keep the
 reference's semantics; the per-pixel work (normalise, cell lookup, 8-corner trilinear blend, strength blend)

@@ -1,4 +1,4 @@
-"""Resample helpers around the reference's Video Enhance nodes, same names and signatures, on one sm_100a gather kernel.
+"""Resample helpers around the reference's Video Enhance nodes, same names and signatures, on one sm_90a gather kernel.
 
 Reference: VRGDG_VideoEnhanceNodes.py (_interpolation :45-51, _resize_batch :54-86, _restore_batch :89-106, the restore blend of
 VRGDG_VideoEnhanceRestore :404-418).  F.interpolate + crop / F.pad + clamp become ONE launch (vrgdg_resize): the fit mode only

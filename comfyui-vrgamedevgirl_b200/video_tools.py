@@ -1,4 +1,4 @@
-"""Tensor-math helpers of the reference's file->file video paths, same names and signatures, on sm_100a kernels.
+"""Tensor-math helpers of the reference's file->file video paths, same names and signatures, on sm_90a kernels.
 
 Reference: VRGDG_LUTVideoTools.py (_apply_lut_tensor :172-185, _apply_film_grain_tensor :262-277, uint8 codecs :736-752)
 and VRGDG_StandaloneVideoEnhancerNodes.py (_auto_batch_size :200-210, _apply_unsharp :233-258, _apply_seeded_grain :261-275,

@@ -1,5 +1,5 @@
 /*
- * vrgdg_b200.h — C ABI of libvrgdg_b200.so: B200 (sm_100a) kernels for the per-pixel video
+ * vrgdg_b200.h — C ABI of libvrgdg_b200.so: H100 (sm_90a) kernels for the per-pixel video
  * post-processing hot path of the comfyui-vrgamedevgirl node pack.
  *
  * The reference is pure Python (no FFI of its own); each entry point below replaces the tensor
@@ -94,7 +94,7 @@ VRGDG_API const char* vrgdg_last_tile_path(void);
 VRGDG_API int64_t vrgdg_lut3d_packed_bytes(int lut_size);
 /* lut: device [S,S,S,3] fp32 (reference layout); packed: device buffer of vrgdg_lut3d_packed_bytes(S), 32-byte aligned.
  * Entry (b,g,r) of the packed table = the 8 corners of the cell whose origin is (b,g,r) (neighbours clamped to S-1), 24 floats
- * = 96 bytes: a pixel's whole trilinear stencil arrives with three consecutive 256-bit loads.  The buffer holds TWO tables of
+ * = 96 bytes: a pixel's whole trilinear stencil arrives with three consecutive 32-byte sectors.  The buffer holds TWO tables of
  * S^3 x 96 bytes: the corner cells (every exact entry point: bit-identical lookups) followed by the same cells as coefficients
  * of the trilinear polynomial (differences of the corners formed in double, rounded once), which the chains that draw their own
  * grain evaluate with 7 FMAs per channel (fast arithmetic, a few 1e-8 of the table values away from the corner form). */

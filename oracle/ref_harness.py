@@ -1,8 +1,9 @@
-"""Executes the REFERENCE's own source for the hot path — TEST INFRASTRUCTURE, container-only.
+"""Executes the REFERENCE's own source for the hot path — TEST INFRASTRUCTURE, optional.
 
-/root/reference exists only in the build container (never on the GPU box), so nothing under `-m gpu`,
-smoke() or bench.py may import this module.  It is used by tests/golden/make_golden.py to freeze golden
-vectors and by tests/test_oracle_golden.py (skipped when the tree is absent) to pin oracle/vrgdg_oracle.py.
+The reference (a checkout of vrgamegirl19/comfyui-vrgamedevgirl) is not part of this repository: point
+VRGDG_REFERENCE_ROOT at one to use this module.  Nothing under `-m gpu`, smoke() or bench.py imports it.  It is
+used by tests/golden/make_golden.py to freeze the golden vectors the suite compares against, and by
+tests/test_oracle_golden.py (skipped without a reference checkout) to pin oracle/vrgdg_oracle.py on fresh inputs.
 
 Technique = the reference's own tests (tests/test_standalone_video_enhancer.py:19-36): ast.parse the file,
 keep the wanted top-level definitions, exec them in a namespace of stand-ins for what ComfyUI provides.
@@ -19,11 +20,11 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-REFERENCE_ROOT = os.environ.get("VRGDG_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("VRGDG_REFERENCE_ROOT", "")
 
 
 def available():
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, "nodes.py"))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, "nodes.py"))
 
 
 def _extract(path, names, namespace):

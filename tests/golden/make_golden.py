@@ -1,7 +1,7 @@
 """Freezes golden input/output vectors by EXECUTING THE REFERENCE'S OWN SOURCE (oracle/ref_harness.py).
 
-Run in the build container only (needs /root/reference):   python tests/golden/make_golden.py
-The .npz / .json files it writes are committed; GPU-box tests read them and never touch /root/reference.
+Needs a checkout of the reference:   VRGDG_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py
+The .npz / .json files it writes are committed; the tests read them and never need the reference.
 """
 import hashlib
 import json

@@ -61,12 +61,13 @@ def test_version_and_error_channel_without_gpu(pkg):
 
 
 def test_sass_contains_tma_and_no_legacy_tensor_paths(pkg):
-    """sm_100a only; the tile kernels use TMA (UTMALDG) + mbarrier (SYNCS); nothing routes through HMMA."""
+    """sm_90a only; the tile kernels use TMA (UTMALDG) + mbarrier (SYNCS); nothing routes through HMMA."""
     cuobjdump = "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not installed")
     lst = subprocess.run([cuobjdump, "-lelf", pkg._native.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in lst and "sm_90" not in lst and "sm_80" not in lst
+    archs = set(re.findall(r"\.(sm_\w+)\.cubin", lst))
+    assert archs == {"sm_90a"}, archs
 
 
 def test_header_is_plain_c_and_matches_the_ctypes_structs(pkg, tmp_path):

@@ -189,8 +189,8 @@ def test_div_const_keeps_infinities(hostcheck):
 
 def test_div_const_is_the_correctly_rounded_quotient(hostcheck):
     """div_const<D> (3 instructions: q = a*r, q' = fma(fma(-D, q, a), r, q)) against IEEE division on 8 M random finite bit patterns per
-    divisor plus the special values; the GPU-side exhaustive run over all 2^32 patterns is tools/divconst_check.cu
-    (profiles/r01_final_v2/divconst_exhaustive_check.jsonl).  The one representational difference: -0.0 -> +0.0."""
+    divisor plus the special values; the GPU-side exhaustive run over all 2^32 patterns is tools/divconst_check.cu.
+    The one representational difference: -0.0 -> +0.0."""
     hostcheck.hc_div_const.argtypes = [vp, vp, i64, ci]
     rng = np.random.default_rng(5)
     bits = rng.integers(0, 2 ** 32, size=8_000_000, dtype=np.uint64).astype(np.uint32)

@@ -1,5 +1,5 @@
 // tools/lut_bench.cu — exploration micro-benchmark for the 3D-LUT gather (not part of the product).
-// Build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o gpurun_out/lut_bench tools/lut_bench.cu
+// Build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o tools/lut_bench.bin tools/lut_bench.cu
 // Compares table layouts / load widths / smem residency on white and natural-like frames.
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -69,8 +69,9 @@ __device__ __forceinline__ void eval_f4(LD ld, int S, float& r, float& g, float&
 struct F8 { float4 a, b; };
 __device__ __forceinline__ F8 ld256(const float* p) {
   F8 v;
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v.a.x), "=f"(v.a.y), "=f"(v.a.z), "=f"(v.a.w), "=f"(v.b.x), "=f"(v.b.y), "=f"(v.b.z), "=f"(v.b.w) : "l"(p));
+  // sm_90 has no 256-bit load: one 32-byte sector as two 128-bit non-coherent loads
+  asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.a.x), "=f"(v.a.y), "=f"(v.a.z), "=f"(v.a.w) : "l"(p));
+  asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+16];" : "=f"(v.b.x), "=f"(v.b.y), "=f"(v.b.z), "=f"(v.b.w) : "l"(p));
   return v;
 }
 __device__ __forceinline__ F8 ld2x128(const float* p) {

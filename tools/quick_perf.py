@@ -17,7 +17,7 @@ CLK = Clocks(0)
 
 nv, ops = pkg._native, pkg.ops
 dev = torch.device("cuda", 0)
-PEAK = 6573.5
+PEAK = 3350.0     # GB/s: H100 SXM data sheet (HBM3)
 
 
 LAST_CLOCKS = [None]

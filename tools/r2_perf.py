@@ -18,7 +18,7 @@ from _clocks import Clocks  # noqa: E402
 
 nv, ops = pkg._native, pkg.ops
 dev = torch.device("cuda", 0)
-PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0   # H100 SXM data sheet
 CLK = Clocks(0)
 
 
