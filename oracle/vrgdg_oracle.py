@@ -559,6 +559,42 @@ def chain_full(images, noise, grain_intensity, saturation_mix, reference_image, 
     return unsharp_numpy(x, sharpen_strength)
 
 
+# (op, border) of a chain's stencil stage -> the reference function that owns that pair (VRGDG_STENCIL_*, VRGDG_BORDER_*)
+CHAIN_STENCILS = {(1, 0): unsharp_numpy, (1, 1): unsharp_torch, (2, 0): laplacian_numpy, (3, 1): laplacian_torch,
+                  (4, 0): sobel_numpy, (5, 1): sobel_torch}
+
+
+def chain_compose(x, *, grain=None, colormatch=None, lut=None, stencil=None, post_grain=None, z=None, post_z=None):
+    """The fused chain (vrgdg_chain_desc) as the reference nodes applied one after another, each stage optional:
+    grain -> colour match (statistics of the GRAINED frames) -> 3D LUT -> 3x3 stencil -> post grain.
+      grain / post_grain: dict(intensity, saturation_mix), drawing N(0,1) from z / post_z (fp32, [B,H,W,3], RGB)
+      colormatch:         dict(reference_image=[1,h,w,3] fp32, strength)
+      lut:                dict(lut_data=parse_cube(...), strength 0..10)
+      stencil:            dict(op, border, strength); (op, border) must be a key of CHAIN_STENCILS
+    x: fp32 frames; fp16 / bf16 frames go through on the up-cast input and are rounded once at the end; uint8 BGR frames go
+    through the reference's wire format (frames_to_tensor -> stages -> tensor_to_frames)."""
+    if x.dtype == torch.uint8:
+        return torch.from_numpy(tensor_to_frames(chain_compose(frames_to_tensor(x.numpy()), grain=grain, colormatch=colormatch, lut=lut,
+                                                               stencil=stencil, post_grain=post_grain, z=z, post_z=post_z)))
+    if x.dtype != torch.float32:
+        return chain_compose(x.float(), grain=grain, colormatch=colormatch, lut=lut, stencil=stencil, post_grain=post_grain, z=z,
+                             post_z=post_z).to(x.dtype)
+    if grain is not None:
+        x = film_grain(x, grain["intensity"], grain["saturation_mix"], batch_size=0, noise=z)
+    if colormatch is not None:
+        x = color_match(x, colormatch["reference_image"], colormatch["strength"], batch_size=1)
+    if lut is not None:
+        x = apply_lut(x, lut["lut_data"], lut["strength"])
+    if stencil is not None:
+        key = (int(stencil["op"]), int(stencil["border"]))
+        if key not in CHAIN_STENCILS:
+            raise ValueError("no reference function owns stencil op %d with border %d" % key)
+        x = CHAIN_STENCILS[key](x, stencil["strength"])
+    if post_grain is not None:
+        x = film_grain(x, post_grain["intensity"], post_grain["saturation_mix"], batch_size=0, noise=post_z)
+    return x.contiguous()
+
+
 def hist_counts(images):
     """256-bin counts per frame and RGB channel: bin = min(floor(clip(v,0,1) * 256), 255) evaluated in fp32.  int64 [B,3,256]."""
     x = images.detach().cpu().float().numpy()
