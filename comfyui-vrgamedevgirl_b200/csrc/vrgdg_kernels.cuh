@@ -111,20 +111,27 @@ __device__ __forceinline__ void process_pixel(const PointParams& P, const CmFold
   }
 }
 
-// two pixels at once: all per-pixel stages up to the LUT, then BOTH gathers issued before either is consumed
+// the LUT stage of a pixel pair p[0..5] (RGB), strength blend included: BOTH gathers are issued before either is consumed.
+// LANE_PAIR: the sector loads are split between lane pairs (lut_eval_lane_pair): every lane of a full warp must call it.
+template <bool EXACT, bool LANE_PAIR>
+__device__ __forceinline__ void lut_pair(const PointParams& P, float* p) {
+  constexpr bool POLY = !EXACT && VRGDG_LUT_POLY;
+  float x[6] = {p[0], p[1], p[2], p[3], p[4], p[5]};
+  if (LANE_PAIR) lut_eval_lane_pair<POLY, EXACT>(P.lut, p, p + 3);
+  else if (POLY) lutp_eval2(P.lut, p, p + 3);
+  else lut3d_eval2<EXACT>(P.lut, p, p + 3);
+  if (P.lut.blend < 1.0f) {
+#pragma unroll
+    for (int i = 0; i < 6; ++i) p[i] = lut_blend<EXACT>(x[i], p[i], P.lut.blend, P.lut.one_minus_blend);
+  }
+}
+
+// two pixels at once: all per-pixel stages up to the LUT, then the LUT stage of both
 template <int MASK, bool EXACT>
 __device__ __forceinline__ void process_pair(const PointParams& P, const CmFold& cmf, const float* z, float* p) {
   process_pixel<(MASK & ~ST_LUT), EXACT>(P, cmf, z[0], z[1], z[2], p[0], p[1], p[2]);
   process_pixel<(MASK & ~ST_LUT), EXACT>(P, cmf, z[3], z[4], z[5], p[3], p[4], p[5]);
-  if (MASK & ST_LUT) {
-    float x[6] = {p[0], p[1], p[2], p[3], p[4], p[5]};
-    if (EXACT || !VRGDG_LUT_POLY) lut3d_eval2<EXACT>(P.lut, p, p + 3);
-    else lutp_eval2(P.lut, p, p + 3);
-    if (P.lut.blend < 1.0f) {
-#pragma unroll
-      for (int i = 0; i < 6; ++i) p[i] = lut_blend<EXACT>(x[i], p[i], P.lut.blend, P.lut.one_minus_blend);
-    }
-  }
+  if (MASK & ST_LUT) lut_pair<EXACT, false>(P, p);
 }
 
 // =====================================================================================================
@@ -358,7 +365,7 @@ template <typename T, int MASK> struct TileCfg {
   // cap (65536 / (LB_THREADS * MINB)) below the 128 that two 256-thread CTAs would allow, which leaves room in the register file for
   // the statistics blocks of the NEXT frame group next to two resident tile CTAs (pipelined colour-match schedule, vrgdg_abi.cu).
   // 256 (104-109 registers) fits one 128-thread statistics block beside two tile CTAs, 320 (91-94 registers) two, 352 (80 registers)
-  // three or four.  At 80 registers the sm_90a LUT tile kernels spill 12-168 bytes per thread (ptxas -v).  352 was chosen by a sweep
+  // three or four.  At 80 registers the sm_90a LUT tile kernels spill 12-108 bytes per thread (ptxas -v).  352 was chosen by a sweep
   // on an earlier GPU with the same register file and shared memory per SM and has not been re-swept on H100.
 #ifndef VRGDG_HEAVY_LB
 #define VRGDG_HEAVY_LB 352
@@ -728,12 +735,16 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
       const bool has_ext = GRAIN && (P.ext_noise != nullptr);
       const GrainFrame pgf = grain_frame(Q.pseed, Q.pframe0, frame, Q.pseed_mode);
       const int pair0 = x0e / 6 - 1;                        // pair holding the left halo pixel (x0e is a multiple of TXE, TXE of 6)
-      for (int i = tid; i < ROWS * C::PAIRS; i += NT) {
+      constexpr int TASKS = ROWS * C::PAIRS;
+      // whole warps walk the tasks (the LUT gather shuffles between lanes): a lane past the last task computes on zeros and stores nothing
+      for (int i0 = tid & ~31; i0 < TASKS; i0 += NT) {
+        const int i = i0 + (tid & 31);
+        const bool task = i < TASKS;
         const int r = i / C::PAIRS, kx = i - r * C::PAIRS;
         const int y = y0 - 1 + r, pair = pair0 + kx;
         const int pxa = pair * 2;
         const int so = r * BX + PADL - 6 + 6 * kx;          // smem element of pixel a (outside the box for kx == 0)
-        const bool rowin = (y >= 0 && y < Q.H);
+        const bool rowin = task && (y >= 0 && y < Q.H);
         const bool need_a = (kx > 0), need_b = (kx < C::PAIRS - 1);
         const bool in_a = need_a && rowin && pxa >= 0 && pxa < Q.W;
         const bool in_b = need_b && rowin && pxa + 1 >= 0 && pxa + 1 < Q.W;
@@ -751,10 +762,11 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
             gz[0] = BGR ? b0 : r0; gz[1] = g0; gz[2] = BGR ? r0 : b0;
             gz[3] = BGR ? b1 : r1; gz[4] = g1; gz[5] = BGR ? r1 : b1;
           }
-          pair_store6(gplane + so, kx > 0, gz);
+          if (task) pair_store6(gplane + so, kx > 0, gz);
         }
         if ((MASK & ST_PRE) == 0 && !WORK) continue;               // nothing to do to the pixel values themselves
         float e[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        float p[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};               // RGB for the stages
         if (in_a | in_b) {
           pair_load6<T>(raw + so, kx > 0, e);
           float z[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -769,13 +781,16 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
           }
           // both pixels go through the stages unconditionally (their 2 x 3 LUT loads are then in flight together; a pixel
           // outside the image computes on staged zeros and is discarded) - the branchy form serialised the two gathers
-          float p[6] = {e[BGR ? 2 : 0], e[1], e[BGR ? 0 : 2], e[BGR ? 5 : 3], e[4], e[BGR ? 3 : 5]};     // RGB for the stages
-          process_pair<MASK, EXACT>(P, cmf, z, p);
+          p[0] = e[BGR ? 2 : 0]; p[1] = e[1]; p[2] = e[BGR ? 0 : 2]; p[3] = e[BGR ? 5 : 3]; p[4] = e[4]; p[5] = e[BGR ? 3 : 5];
+          process_pair<(MASK & ~ST_LUT), EXACT>(P, cmf, z, p);
+        }
+        if (MASK & ST_LUT) lut_pair<EXACT, true>(P, p);           // every lane: lanes without pixels in the image serve their partner
+        if (in_a | in_b) {
           if (in_a) { e[BGR ? 2 : 0] = p[0]; e[1] = p[1]; e[BGR ? 0 : 2] = p[2]; } else if (WORK) { e[0] = 0.f; e[1] = 0.f; e[2] = 0.f; }
           if (in_b) { e[BGR ? 5 : 3] = p[3]; e[4] = p[4]; e[BGR ? 3 : 5] = p[5]; } else if (WORK) { e[3] = 0.f; e[4] = 0.f; e[5] = 0.f; }
         }
         if constexpr (WORK) {
-          pair_store6(work + so, kx > 0, e);                       // zeros for pixels outside the image (memory channel order kept)
+          if (task) pair_store6(work + so, kx > 0, e);             // zeros for pixels outside the image (memory channel order kept)
         } else {
           if (in_a | in_b) pair_store6(reinterpret_cast<float*>(raw) + so, kx > 0, e);   // in place; untouched pixels keep their staged value
         }

@@ -222,10 +222,12 @@ VRGDG_HD void grain_blend_fast(float& r, float& g, float& b, float zr, float zg,
 
 // ---- 3D LUT trilinear: VRGDG_IV_Adjustments.py:293-336 ------------------------------------------
 // Device table layout ("cell table", built by lut_pack_entry / vrgdg_lut3d_pack): one 96-byte entry per cell origin
-//   entry (b,g,r) = rgb x { c000 c100 c010 c110 c001 c101 c011 c111 },  cXYZ = lut[min(b+Z,S-1), min(g+Y,S-1), min(r+X,S-1), :]
-// (channel-planar: one 32-byte sector per output channel) so a pixel fetches its 8 corners (24 floats) from THREE sectors at
-// consecutive addresses (lut_load8) instead of 24 scalar loads - or three lanes fetch one sector each.  The gather is bound by L1 tag
-// lookups per divergent lane, not by bytes: 3 sectors per pixel beat both a 32-byte r-pair table (4 per pixel) and scalar loads.
+//   entry (b,g,r) = rgb x { c000 c001 c010 c011 | c100 c101 c110 c111 },  cXYZ = lut[min(b+Z,S-1), min(g+Y,S-1), min(r+X,S-1), :]
+// (channel-planar: one 32-byte sector per output channel, corner cXYZ in slot 4X + 2Y + Z) so a pixel fetches its 8 corners (24 floats)
+// from THREE sectors at consecutive addresses (lut_load8) instead of 24 scalar loads.  The gather is bound by L1 wavefronts per
+// divergent lane, not by bytes: 3 sectors per pixel beat both a 32-byte r-pair table (4 per pixel) and scalar loads.  Each 16-byte
+// half of a sector is one r side of the cell (X = 0 below, X = 1 above) and interpolates along b and g on its own (lut_half), so two
+// lanes can split a sector between them (lut_eval_lane_pair, the tile kernels' pre-stage).
 struct LutParams {
   const float* lut;      // cell table, S*S*S*24 floats: per cell three 32-byte sectors (R, G, B), 8 corners each
   const float* lutp;     // polynomial cell table (fast arithmetic only, see lutp_* below), same shape as `lut`
@@ -238,29 +240,36 @@ struct LutParams {
 
 constexpr int LUT_CELL_FLOATS = 24;
 
+struct F4 { float v[4]; };
 struct F8 { float v[8]; };
 
-// One 32-byte sector as two 128-bit non-coherent loads (LDG.E.128.CONSTANT): sm_90 has no 256-bit load, and both halves hit
-// the same sector, so the L2 -> L1 traffic per corner set is unchanged.
-VRGDG_HD F8 lut_load8(const float* p) {
-  F8 q;
+// One 16-byte half sector as a 128-bit non-coherent load (LDG.E.128.CONSTANT).
+VRGDG_HD F4 lut_load4(const float* p) {
+  F4 q;
 #if defined(__CUDA_ARCH__)
   asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];"
       : "=f"(q.v[0]), "=f"(q.v[1]), "=f"(q.v[2]), "=f"(q.v[3]) : "l"(p));
-  asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+16];"
-      : "=f"(q.v[4]), "=f"(q.v[5]), "=f"(q.v[6]), "=f"(q.v[7]) : "l"(p));
 #else
-  for (int i = 0; i < 8; ++i) q.v[i] = p[i];
+  for (int i = 0; i < 4; ++i) q.v[i] = p[i];
 #endif
   return q;
 }
 
-// one cell-table entry from the reference-layout table [S][S][S][3]
+// One 32-byte sector as two 128-bit loads: sm_90 has no 256-bit load.  Each of the two is a request of its own in the L1 data
+// pipe, so a warp's divergent gather of whole sectors this way costs two instructions of up to 32 distinct lines each.
+VRGDG_HD F8 lut_load8(const float* p) {
+  const F4 lo = lut_load4(p), hi = lut_load4(p + 4);
+  F8 q;
+  for (int i = 0; i < 4; ++i) { q.v[i] = lo.v[i]; q.v[4 + i] = hi.v[i]; }
+  return q;
+}
+
+// one cell-table entry from the reference-layout table [S][S][S][3]; corner cXYZ in slot 4X + 2Y + Z
 VRGDG_HD void lut_pack_entry(const float* lut3, int S, int b, int g, int r, float* dst24) {
   const int b1 = (b + 1 < S) ? b + 1 : S - 1, g1 = (g + 1 < S) ? g + 1 : S - 1, r1 = (r + 1 < S) ? r + 1 : S - 1;
-  const int cb[8] = {b, b, b, b, b1, b1, b1, b1};
+  const int cb[8] = {b, b1, b, b1, b, b1, b, b1};
   const int cg[8] = {g, g, g1, g1, g, g, g1, g1};
-  const int cr[8] = {r, r1, r, r1, r, r1, r, r1};
+  const int cr[8] = {r, r, r, r, r1, r1, r1, r1};
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const float* a = lut3 + ((size_t)(cb[k] * S + cg[k]) * S + cr[k]) * 3;
@@ -285,16 +294,21 @@ VRGDG_HD float lerp_ref(float a, float b, float f, float omf) {
   return fmaf(f, b - a, a);                           // contracted form for fused chains (<= 2e-7 away)
 }
 
-// one channel from its sector q = {c000 c100 c010 c110 c001 c101 c011 c111} (cXYZ: X = r, Y = g, Z = b neighbour), :318-339
+// The trilinear interpolation of :318-339 split at its last step: lut_half interpolates one r side of the cell,
+// h = {cX00 cX01 cX10 cX11} (cXYZ: X = r, Y = g, Z = b neighbour), along b and then g; lut_combine interpolates the two sides along r.
+template <bool EXACT>
+VRGDG_HD float lut_half(const float* h, float fg, float fb, float omg, float omb) {
+  const float cx0 = lerp_ref<EXACT>(h[0], h[1], fb, omb);         // cX00*(1-fb) + cX01*fb
+  const float cx1 = lerp_ref<EXACT>(h[2], h[3], fb, omb);         // cX10, cX11
+  return lerp_ref<EXACT>(cx0, cx1, fg, omg);
+}
+template <bool EXACT>
+VRGDG_HD float lut_combine(float c0, float c1, float fr, float omr) { return clamp01(lerp_ref<EXACT>(c0, c1, fr, omr)); }
+
+// one channel from its sector q = {c000 c001 c010 c011 c100 c101 c110 c111}
 template <bool EXACT>
 VRGDG_HD float lut_channel(const F8& q, float fr, float fg, float fb, float omr, float omg, float omb) {
-  const float c00 = lerp_ref<EXACT>(q.v[0], q.v[4], fb, omb);     // c000*(1-fb) + c001*fb
-  const float c01 = lerp_ref<EXACT>(q.v[2], q.v[6], fb, omb);     // c010, c011
-  const float c10 = lerp_ref<EXACT>(q.v[1], q.v[5], fb, omb);     // c100, c101
-  const float c11 = lerp_ref<EXACT>(q.v[3], q.v[7], fb, omb);     // c110, c111
-  const float c0 = lerp_ref<EXACT>(c00, c01, fg, omg);
-  const float c1 = lerp_ref<EXACT>(c10, c11, fg, omg);
-  return clamp01(lerp_ref<EXACT>(c0, c1, fr, omr));
+  return lut_combine<EXACT>(lut_half<EXACT>(q.v, fg, fb, omg, omb), lut_half<EXACT>(q.v + 4, fg, fb, omg, omb), fr, omr);
 }
 
 template <bool EXACT>
@@ -313,9 +327,8 @@ VRGDG_HD void lut3d_eval(const LutParams& P, float& r, float& g, float& b) {
   b = lut_channel<EXACT>(q2, fr, fg, fb, omr, omg, omb);
 }
 
-// One output channel only: the element-mapped gather of the tile kernels (three lanes of a pixel read the three sectors of
-// one cell, i.e. one or two 128-byte lines per PIXEL instead of three per pixel: the L1 data pipe counts wavefronts per
-// distinct line and instruction; tools/lut_bench.cu compares the two mappings as v10 and v13).
+// One output channel only (an element-mapped gather: three lanes of a pixel read the three sectors of one cell;
+// tools/lut_bench.cu compares that mapping with the per-pixel one as v13 and v10).
 template <bool EXACT>
 VRGDG_HD float lut3d_eval_channel(const LutParams& P, float r, float g, float b, int ch) {
   int r0, r1, g0, g1, b0, b1;
@@ -329,17 +342,22 @@ VRGDG_HD float lut3d_eval_channel(const LutParams& P, float r, float g, float b,
 }
 
 // Two pixels at once: both address computations first, then all six sector loads, then the lerps, so that the two
-// gathers overlap (the tile pre-stage is latency-bound on these loads).
+// gathers overlap (the streaming kernels are latency-bound on these loads).
 struct LutCell { const float* p; float fr, fg, fb; };
 
-VRGDG_HD LutCell lut_locate(const LutParams& P, float r, float g, float b) {
+// cell of a pixel as a float offset into the table (< 65^3 * 24) and its fractions
+VRGDG_HD int lut_cell_offset(const LutParams& P, float r, float g, float b, float& fr, float& fg, float& fb) {
   int r0, r1, g0, g1, b0, b1;
-  LutCell c;
-  lut_coord(r, P.dmin[0], P.dspan[0], P.unit_domain != 0, P.smax, P.S, r0, r1, c.fr);
-  lut_coord(g, P.dmin[1], P.dspan[1], P.unit_domain != 0, P.smax, P.S, g0, g1, c.fg);
-  lut_coord(b, P.dmin[2], P.dspan[2], P.unit_domain != 0, P.smax, P.S, b0, b1, c.fb);
+  lut_coord(r, P.dmin[0], P.dspan[0], P.unit_domain != 0, P.smax, P.S, r0, r1, fr);
+  lut_coord(g, P.dmin[1], P.dspan[1], P.unit_domain != 0, P.smax, P.S, g0, g1, fg);
+  lut_coord(b, P.dmin[2], P.dspan[2], P.unit_domain != 0, P.smax, P.S, b0, b1, fb);
   (void)r1; (void)g1; (void)b1;
-  c.p = P.lut + (size_t)((b0 * P.S + g0) * P.S + r0) * LUT_CELL_FLOATS;
+  return ((b0 * P.S + g0) * P.S + r0) * LUT_CELL_FLOATS;
+}
+
+VRGDG_HD LutCell lut_locate(const LutParams& P, float r, float g, float b) {
+  LutCell c;
+  c.p = P.lut + lut_cell_offset(P, r, g, b, c.fr, c.fg, c.fb);
   return c;
 }
 
@@ -367,7 +385,7 @@ VRGDG_HD void lut3d_eval2(const LutParams& P, float* a, float* b) {
 //   k_000 = c000, k_100 = c100 - c000, k_010 = c010 - c000, k_110 = c110 - c100 - c010 + c000, ...  (differences along r, g, b)
 // evaluated as a nested Horner form with 7 FMAs per channel (the corner form needs 7 lerps = 14 instructions):
 //   v = (k000 + fb k001 + fg (k010 + fb k011)) + fr (k100 + fb k101 + fg (k110 + fb k111)).
-// Same 96-byte channel-planar cell, coefficient k_XYZ in the slot of corner cXYZ; three sector loads per pixel as before.
+// Same 96-byte channel-planar cell, coefficient k_XYZ in the slot of corner cXYZ (4X + 2Y + Z); three sector loads per pixel as before.
 // The coefficients are formed in double from the fp32 corners and rounded once; cell index and fractions are the exact path's.
 // Difference to the exact interpolation: a few 1e-8 of the table values (rounding of coefficients and FMAs).
 VRGDG_HD void lutp_pack_entry(const float* lut3, int S, int b, int g, int r, float* dst24) {
@@ -378,8 +396,10 @@ VRGDG_HD void lutp_pack_entry(const float* lut3, int S, int b, int g, int r, flo
     double k[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) k[i] = (double)c[8 * ch + i];
+    // Moebius transform: slot i (bit set) -= slot i without that bit.  Differences along r (bit 4) first, then g, then b: the order in
+    // which the double sums are formed stays the same whatever the slot order (a difference of far-apart values is not exact in double).
 #pragma unroll
-    for (int bit = 1; bit < 8; bit <<= 1) {          // Moebius transform: slot i (bit set) -= slot i without that bit
+    for (int bit = 4; bit >= 1; bit >>= 1) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) if (i & bit) k[i] -= k[i ^ bit];
     }
@@ -388,11 +408,14 @@ VRGDG_HD void lutp_pack_entry(const float* lut3, int S, int b, int g, int r, flo
   }
 }
 
-// one channel from its coefficient sector q (slot XYZ: X = r, Y = g, Z = b exponent; slot index = X + 2 Y + 4 Z)
+// Horner form split like lut_half / lut_combine: lutp_half evaluates one r side h = {kX00 kX01 kX10 kX11},
+// A = k000 + fb k001 + fg (k010 + fb k011) for X = 0 and B = k100 + ... for X = 1; lutp_combine returns A + fr B.
+VRGDG_HD float lutp_half(const float* h, float fg, float fb) { return fmaf(fg, fmaf(fb, h[3], h[2]), fmaf(fb, h[1], h[0])); }
+VRGDG_HD float lutp_combine(float a, float b, float fr) { return clamp01(fmaf(fr, b, a)); }
+
+// one channel from its coefficient sector q (slot 4X + 2Y + Z holds k_XYZ: X = r, Y = g, Z = b exponent)
 VRGDG_HD float lutp_channel(const F8& q, float fr, float fg, float fb) {
-  const float a0 = fmaf(fb, q.v[4], q.v[0]), b0 = fmaf(fb, q.v[5], q.v[1]);
-  const float a1 = fmaf(fb, q.v[6], q.v[2]), b1 = fmaf(fb, q.v[7], q.v[3]);
-  return clamp01(fmaf(fr, fmaf(fg, b1, b0), fmaf(fg, a1, a0)));
+  return lutp_combine(lutp_half(q.v, fg, fb), lutp_half(q.v + 4, fg, fb), fr);
 }
 
 VRGDG_HD LutCell lutp_locate(const LutParams& P, float r, float g, float b) {
@@ -412,6 +435,61 @@ VRGDG_HD void lutp_eval2(const LutParams& P, float* a, float* b) {
   a[0] = lutp_channel(a0, ca.fr, ca.fg, ca.fb); a[1] = lutp_channel(a1, ca.fr, ca.fg, ca.fb); a[2] = lutp_channel(a2, ca.fr, ca.fg, ca.fb);
   b[0] = lutp_channel(b0, cb.fr, cb.fg, cb.fb); b[1] = lutp_channel(b1, cb.fr, cb.fg, cb.fb); b[2] = lutp_channel(b2, cb.fr, cb.fg, cb.fb);
 }
+
+#if defined(__CUDACC__)
+// The lookup of a pixel pair per lane, with the sector loads split between lane pairs (the tile kernels' pre-stage).  Lanes 2i and
+// 2i+1 hand each other the cell offset, fg and fb of their pixels and walk the lane pair's 4 pixels x 3 channels together: per
+// pixel and channel the even lane loads the r0 half and the odd lane the r1 half of the SAME sector, so a warp load instruction
+// touches at most 16 sectors (32 with whole sectors per lane: lut_load8) and each sector is requested once.  Each lane
+// interpolates its half (lut_half / lutp_half), one shuffle per pixel and channel hands it to the pixel's owner, which finishes
+// along r with its own fr.  Results are bit-identical to lut3d_eval2 / lutp_eval2.
+// Needs a full, converged warp: lanes without a pixel pair pass any values (a valid cell is always addressed) and discard the result.
+// POLY: coefficient cells (lutp_*), else corner cells (lut_*).  a = pixel 0 (r, g, b), b = pixel 1, both in / out.
+template <bool POLY, bool EXACT>
+__device__ __forceinline__ void lut_eval_lane_pair(const LutParams& P, float* a, float* b) {
+  const unsigned FULL = 0xffffffffu;
+  const bool odd = (threadIdx.x & 1) != 0;
+  float fr[2], fg[2], fb[2];
+  int cell[2];
+  cell[0] = lut_cell_offset(P, a[0], a[1], a[2], fr[0], fg[0], fb[0]);
+  cell[1] = lut_cell_offset(P, b[0], b[1], b[2], fr[1], fg[1], fb[1]);
+  // the lane pair's 4 pixels in one order on both lanes: the even lane's two, then the odd lane's two
+  int qc[4];
+  float qg[4], qb[4];
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const int pc = __shfl_xor_sync(FULL, cell[k], 1);
+    const float pg = __shfl_xor_sync(FULL, fg[k], 1), pb = __shfl_xor_sync(FULL, fb[k], 1);
+    qc[k] = odd ? pc : cell[k];     qg[k] = odd ? pg : fg[k];     qb[k] = odd ? pb : fb[k];
+    qc[2 + k] = odd ? cell[k] : pc; qg[2 + k] = odd ? fg[k] : pg; qb[2 + k] = odd ? fb[k] : pb;
+  }
+  const float* tab = (POLY ? P.lutp : P.lut) + (odd ? 4 : 0);
+  F4 q[4][3];
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) q[k][ch] = lut_load4(tab + qc[k] + 8 * ch);
+  float h[4][3];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float omg = subx(1.0f, qg[k]), omb = subx(1.0f, qb[k]);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) h[k][ch] = POLY ? lutp_half(q[k][ch].v, qg[k], qb[k]) : lut_half<EXACT>(q[k][ch].v, qg[k], qb[k], omg, omb);
+  }
+  float* px[2] = {a, b};
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const float omr = subx(1.0f, fr[k]);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      const float mine = odd ? h[2 + k][ch] : h[k][ch];
+      const float other = __shfl_xor_sync(FULL, odd ? h[k][ch] : h[2 + k][ch], 1);
+      const float c0 = odd ? other : mine, c1 = odd ? mine : other;
+      px[k][ch] = POLY ? lutp_combine(c0, c1, fr[k]) : lut_combine<EXACT>(c0, c1, fr[k], omr);
+    }
+  }
+}
+#endif
 
 // strength blend of apply_lut (:355-359) on already-rounded LUT output `y` and input `x`
 template <bool EXACT>

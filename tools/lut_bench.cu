@@ -249,6 +249,109 @@ __global__ void __launch_bounds__(256) k_lut_coop(const T* __restrict__ in, T* _
   }
 }
 
+// ---- variant 15: lane-pair split sector.  One lane per PIXEL PAIR as in the product's tile pre-stage; the channel sectors hold the
+// corners in slot 4X + 2Y + Z, so the lower 16 bytes are the r0 half {c000 c001 c010 c011} and the upper 16 bytes the r1 half.
+// Lanes 2i and 2i+1 walk the 4 pixels of the lane pair together: per pixel and channel the even lane loads the lower and the odd lane
+// the upper half of the SAME sector (one LDG.128 per lane: a warp instruction touches at most 16 sectors instead of 32), each
+// interpolates its half along b and g, and one shuffle per pixel and channel hands the partner's half to the pixel's owner. ----
+__device__ __forceinline__ float4 ld128(const float* p) {
+  float4 v;
+  asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+  return v;
+}
+template <typename T>
+__global__ void __launch_bounds__(256) k_lut_pair(const T* __restrict__ in, T* __restrict__ out, int64_t npix, const float* __restrict__ lute, int S) {
+  const unsigned FULL = 0xffffffffu;
+  const float smax = (float)(S - 1);
+  const int odd = threadIdx.x & 1;
+  const int64_t npair = npix / 2;                                         // npix is even
+  const int64_t nround = (npair + 31) / 32;
+  const int64_t warp0 = ((int64_t)blockIdx.x * 256 + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * 256) >> 5;
+  for (int64_t w = warp0; w < nround; w += nwarps) {                     // warp-uniform trip count: the shuffles need full warps
+    const int64_t pp = w * 32 + (threadIdx.x & 31);
+    const bool own = pp < npair;
+    float x[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (own) {
+      const T* s = in + pp * 6;
+#pragma unroll
+      for (int i = 0; i < 6; ++i) x[i] = E<T>::ld(__ldg(s + i));
+    }
+    int cell[2]; float fr[2], fg[2], fb[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      Idx c;
+      coord<false>(x[3 * k], smax, S, c.r0, c.r1, c.fr); coord<false>(x[3 * k + 1], smax, S, c.g0, c.g1, c.fg);
+      coord<false>(x[3 * k + 2], smax, S, c.b0, c.b1, c.fb);
+      cell[k] = ((c.b0 * S + c.g0) * S + c.r0) * 24; fr[k] = c.fr; fg[k] = c.fg; fb[k] = c.fb;
+    }
+    int qc[4]; float qg[4], qb[4];                                        // the lane pair's 4 pixels: even lane's two, then odd lane's two
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int pc = __shfl_xor_sync(FULL, cell[k], 1);
+      const float pg = __shfl_xor_sync(FULL, fg[k], 1), pb = __shfl_xor_sync(FULL, fb[k], 1);
+      qc[k] = odd ? pc : cell[k]; qg[k] = odd ? pg : fg[k]; qb[k] = odd ? pb : fb[k];
+      qc[2 + k] = odd ? cell[k] : pc; qg[2 + k] = odd ? fg[k] : pg; qb[2 + k] = odd ? fb[k] : pb;
+    }
+    const float* base = lute + 4 * odd;
+    float4 q[4][3];
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) q[k][ch] = ld128(base + qc[k] + 8 * ch);
+    float h[4][3];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float omb = 1.f - qb[k], omg = 1.f - qg[k];
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const float4 a = q[k][ch];
+        h[k][ch] = lerp1<true>(lerp1<true>(a.x, a.y, qb[k], omb), lerp1<true>(a.z, a.w, qb[k], omb), qg[k], omg);
+      }
+    }
+    float o[6];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const float omr = 1.f - fr[k];
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const float mine = odd ? h[2 + k][ch] : h[k][ch];
+        const float other = __shfl_xor_sync(FULL, odd ? h[k][ch] : h[2 + k][ch], 1);
+        o[3 * k + ch] = clamp01(lerp1<true>(odd ? other : mine, odd ? mine : other, fr[k], omr));
+      }
+    }
+    if (own) {
+      T* d = out + pp * 6;
+#pragma unroll
+      for (int i = 0; i < 6; ++i) d[i] = E<T>::st(o[i]);
+    }
+  }
+}
+
+template <typename T>
+void run_pair(const char* name, const char* tname, const T* in, T* out, int64_t npix, const float* le, int S, int sms, const char* dist, const T* check) {
+  auto kern = k_lut_pair<T>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 0);
+  int occ = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 256, 0));
+  int grid = sms * (occ > 0 ? occ : 1) * 4;
+  cudaEvent_t a, b; CK(cudaEventCreate(&a)); CK(cudaEventCreate(&b));
+  for (int i = 0; i < 2; ++i) kern<<<grid, 256>>>(in, out, npix, le, S);
+  CK(cudaDeviceSynchronize());
+  float best = 1e9f;
+  for (int i = 0; i < 5; ++i) {
+    CK(cudaEventRecord(a)); kern<<<grid, 256>>>(in, out, npix, le, S); CK(cudaEventRecord(b)); CK(cudaEventSynchronize(b));
+    float ms; CK(cudaEventElapsedTime(&ms, a, b)); best = fminf(best, ms);
+  }
+  size_t n = 3 << 18;
+  std::vector<T> h1(n), h2(n);
+  CK(cudaMemcpy(h1.data(), out, n * sizeof(T), cudaMemcpyDeviceToHost)); CK(cudaMemcpy(h2.data(), check, n * sizeof(T), cudaMemcpyDeviceToHost));
+  double md = 0; for (size_t i = 0; i < n; ++i) md = fmax(md, fabs((double)(float)h1[i] - (double)(float)h2[i]));
+  double gpx = npix / (best * 1e-3) / 1e9;
+  printf("{\"variant\": \"%s\", \"dtype\": \"%s\", \"dist\": \"%s\", \"S\": %d, \"ms\": %.4f, \"Gpx/s\": %.1f, \"GB/s\": %.0f, \"occ\": %d, \"maxdiff_vs_v1\": %.3g}\n",
+         name, tname, dist, S, best, gpx, gpx * 6 * sizeof(T), occ, md);
+  fflush(stdout);
+}
+
 template <typename T>
 void run_coop(const char* name, const char* tname, const T* in, T* out, int64_t npix, const float* le, int S, int sms, const char* dist, const T* check) {
   auto kern = k_lut_coop<T>;
@@ -385,14 +488,16 @@ template <typename T> void suite(const char* tname, int sms) {
       hq[i * 16 + 2 * k] = q[0] | (q[1] << 21);
       hq[i * 16 + 2 * k + 1] = (q[1] >> 11) | (q[2] << 10);
     }
-    std::vector<float> he32(n * 32, 0.f), he24(n * 24, 0.f);
+    std::vector<float> he32(n * 32, 0.f), he24(n * 24, 0.f), hs24(n * 24, 0.f);
     for (size_t i = 0; i < n; ++i) for (int k = 0; k < 8; ++k) for (int c = 0; c < 3; ++c) {
       he32[i * 32 + c * 8 + k] = hc[i * 24 + k * 3 + c];
       he24[i * 24 + c * 8 + k] = hc[i * 24 + k * 3 + c];
+      hs24[i * 24 + c * 8 + 4 * (k & 1) + (k & 2) + (k >> 2)] = hc[i * 24 + k * 3 + c];   // corner k = X + 2Y + 4Z -> slot 4X + 2Y + Z
     }
-    float *le32, *le24;
+    float *le32, *le24, *ls24;
     CK(cudaMalloc(&le32, n * 128)); CK(cudaMemcpy(le32, he32.data(), n * 128, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&le24, n * 96)); CK(cudaMemcpy(le24, he24.data(), n * 96, cudaMemcpyHostToDevice));
+    CK(cudaMalloc(&ls24, n * 96)); CK(cudaMemcpy(ls24, hs24.data(), n * 96, cudaMemcpyHostToDevice));
     float* lq; CK(cudaMalloc(&lq, n * 64)); CK(cudaMemcpy(lq, hq.data(), n * 64, cudaMemcpyHostToDevice));
     float *l3, *lp, *lc; float4* l4;
     CK(cudaMalloc(&l3, n * 12)); CK(cudaMalloc(&l4, n * 16)); CK(cudaMalloc(&lp, n * 32)); CK(cudaMalloc(&lc, n * 96));
@@ -416,10 +521,11 @@ template <typename T> void suite(const char* tname, int sms) {
       run_elem<T, 32>("v12_elem_planar_pad128", tname, in, out, npix, le32, S, sms, dist, ref);
       run_elem<T, 24>("v13_elem_planar_96", tname, in, out, npix, le24, S, sms, dist, ref);
       run_coop<T>("v14_pixel_owner_3lane_coop", tname, in, out, npix, le24, S, sms, dist, ref);
+      run_pair<T>("v15_lane_pair_split_sector", tname, in, out, npix, ls24, S, sms, dist, ref);
       if (n * 12 <= 200 * 1024) run<T, 7>("v7_smem_scalar_exact", tname, in, out, npix, l3, l4, lp, S, n * 12, sms, dist, ref);
       if (n * 16 <= 200 * 1024) run<T, 8>("v8_smem_f4_exact", tname, in, out, npix, l3, l4, lp, S, n * 16, sms, dist, ref);
     }
-    cudaFree(l3); cudaFree(l4); cudaFree(lp); cudaFree(lc); cudaFree(lq); cudaFree(le32); cudaFree(le24);
+    cudaFree(l3); cudaFree(l4); cudaFree(lp); cudaFree(lc); cudaFree(lq); cudaFree(le32); cudaFree(le24); cudaFree(ls24);
   }
   cudaFree(in); cudaFree(out); cudaFree(ref);
 }
