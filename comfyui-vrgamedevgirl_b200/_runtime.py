@@ -1,5 +1,10 @@
 """Device policy and host<->device frame streaming shared by the node classes."""
+import os
+import threading
+
 import torch
+
+from .dist import shard_range
 
 
 def _comfy_mm():
@@ -23,6 +28,46 @@ def compute_device(hint=None):
     if not torch.cuda.is_available():
         raise RuntimeError("vrgdg_b200: no CUDA device is available; these nodes are sm_90a kernels and have no CPU path")
     return torch.device("cuda", torch.cuda.current_device())
+
+
+def cuda_device(d):
+    """torch.device of a CUDA device with its index filled in ("cuda" = the current device); anything else is a ValueError."""
+    d = torch.device(d)
+    if d.type != "cuda":
+        raise ValueError("vrgdg_b200: %s is not a CUDA device; these kernels have no CPU path" % d)
+    return d if d.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def devices_from_env():
+    """The CUDA devices VRGDG_DEVICES names for sharding host IMAGE batches, or None when it is unset or empty (the one compute
+    device).  "all" = every visible device of compute capability 9.0; otherwise a comma-separated list of device indices, each
+    visible, of compute capability 9.0 and listed once (a repeated index is most likely a typo for another card)."""
+    raw = os.environ.get("VRGDG_DEVICES", "").strip()
+    if not raw:
+        return None
+    n = torch.cuda.device_count()
+    if raw.lower() == "all":
+        idx = [i for i in range(n) if tuple(torch.cuda.get_device_capability(i)) == (9, 0)]
+        if not idx:
+            raise ValueError("VRGDG_DEVICES=all: none of the %d visible CUDA devices has compute capability 9.0" % n)
+        return [torch.device("cuda", i) for i in idx]
+    idx = []
+    for tok in raw.split(","):
+        tok = tok.strip()
+        try:
+            i = int(tok)
+        except ValueError:
+            raise ValueError("VRGDG_DEVICES=%s: %r is not a device index (use 'all' or a list such as 0,1)" % (raw, tok)) from None
+        if not 0 <= i < n:
+            raise ValueError("VRGDG_DEVICES=%s: there is no device cuda:%d (%d visible)" % (raw, i, n))
+        if i in idx:
+            raise ValueError("VRGDG_DEVICES=%s: device cuda:%d is listed twice" % (raw, i))
+        cap = tuple(torch.cuda.get_device_capability(i))
+        if cap != (9, 0):
+            raise ValueError("VRGDG_DEVICES=%s: device cuda:%d (%s) has compute capability %d.%d; the kernels are sm_90a code for 9.0 only"
+                             % (raw, i, torch.cuda.get_device_name(i), cap[0], cap[1]))
+        idx.append(i)
+    return [torch.device("cuda", i) for i in idx]
 
 
 def result_device(images, numpy_path=False):
@@ -82,12 +127,17 @@ def pipeline_chunk(chunk, frame_bytes, cap=None):
     return max(1, min(int(chunk), cap // max(1, int(frame_bytes))))
 
 
-def _side_streams(dev):
-    """(upload, download) streams of a device, created once (stream creation is not free and ComfyUI calls nodes repeatedly)."""
-    key = (dev.type, dev.index)
-    hit = _SIDE_STREAMS.get(key)
-    if hit is None:
-        hit = _SIDE_STREAMS[key] = (torch.cuda.Stream(dev), torch.cuda.Stream(dev))
+_SIDE_STREAMS_LOCK = threading.Lock()
+
+
+def _side_streams(dev, lane=0):
+    """(upload, download) streams of a device, created once (stream creation is not free and ComfyUI calls nodes repeatedly).
+    `lane` k > 0 is the k-th extra pair of the device, for a sharded call that runs several workers on one card."""
+    key = (dev.type, dev.index, lane)
+    with _SIDE_STREAMS_LOCK:                    # the workers of stream_frames_sharded ask from their own threads
+        hit = _SIDE_STREAMS.get(key)
+        if hit is None:
+            hit = _SIDE_STREAMS[key] = (torch.cuda.Stream(dev), torch.cuda.Stream(dev))
     return hit
 
 
@@ -112,14 +162,15 @@ def bind_to_gpu_numa(device_index):
         return None
 
 
-def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2):
+def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, lane=0):
     """Apply fn(cuda_frames, first_frame_index) -> cuda_frames over src [B,...] in chunks of `chunk` frames (0 / None = all).
 
     CUDA input: chunked as well (the reference bounds device memory with its batch_size widget the same way, nodes.py:49-62);
     one call when the chunk covers the batch.  CPU input: a three-stream pipeline - chunk k+1.. are uploaded into `depth`+1
     reusable staging buffers while chunk k computes and earlier results download; only the last download is waited for.
     Pinned source / result tensors make the copies truly asynchronous (the result is pinned when the source is).  `out`:
-    optional preallocated result on out_device (reused across calls so that pinning cost is paid once)."""
+    optional preallocated result on out_device (reused across calls so that pinning cost is paid once).  `lane`: which pair of
+    the device's upload / download streams carries the copies (stream_frames_sharded gives each worker on a card its own)."""
     B = int(src.shape[0])
     out_device = torch.device(out_device)
     chunk = B if chunk is None or int(chunk) <= 0 else min(int(chunk), max(B, 1))
@@ -154,7 +205,7 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2):
     stage_free = [None, None]
     with torch.cuda.device(dev):
         compute = torch.cuda.current_stream(dev)
-        up, down = _side_streams(dev)
+        up, down = _side_streams(dev, lane)
         if out is None:
             out = torch.empty(src.shape, dtype=src.dtype, pin_memory=_pin_result(src, src.numel() * src.element_size())) if to_cpu \
                 else torch.empty(src.shape, dtype=src.dtype, device=out_device)
@@ -197,4 +248,62 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2):
         ev_last.record(down)
         ev_last.synchronize()                   # the caller reads `out` on the host
         compute.wait_stream(up)
+    return out
+
+
+def shard_plan(n_frames, n_shards):
+    """[(start, stop)] of the contiguous shards stream_frames_sharded cuts a batch into (dist.shard_range: the first shards take the
+    remainder; a shard is empty when there are fewer frames than shards)."""
+    return [shard_range(n_frames, k, n_shards) for k in range(n_shards)]
+
+
+def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None):
+    """stream_frames over several CUDA devices from one process: host frames src [B,...] are cut into one contiguous shard per entry
+    of `devices` (shard_plan), and each non-empty shard runs the stream_frames pipeline on its device in a host thread of its own,
+    writing its slice of one shared result (pinned under stream_frames' rule).
+
+    make_fn(device) -> fn(cuda_frames, first_frame_index) is called once per non-empty shard, in the calling thread and in shard
+    order.  The index handed to fn is absolute (shard start + offset in the shard), so a fn that keys its work by the frame index
+    (grain) or works per frame (everything else here) gives what one device gives.  A device may be listed more than once: its
+    workers get separate upload / download streams.  Kernels go to the calling thread's current stream of each device; a pageable
+    source is staged through pinned buffers of each worker's own.  An exception in a worker is raised here after every worker has
+    finished, and no thread outlives the call.  One device, a CUDA source or a CUDA out_device: one stream_frames call on one
+    device (CUDA batches are not sharded)."""
+    devices = [cuda_device(d) for d in devices]
+    if not devices:
+        raise ValueError("vrgdg_b200: stream_frames_sharded needs at least one CUDA device")
+    out_device = torch.device(out_device)
+    if len(devices) == 1 or src.device.type == "cuda" or out_device.type != "cpu":
+        dev = src.device if src.device.type == "cuda" else devices[0]
+        return stream_frames(src, make_fn(dev), chunk, out_device, dev, out=out)
+    src = src.contiguous()
+    if out is None:
+        out = torch.empty(src.shape, dtype=src.dtype, pin_memory=_pin_result(src, src.numel() * src.element_size()))
+    elif out.shape != src.shape or out.dtype != src.dtype or out.device != out_device:
+        raise ValueError("vrgdg_b200: `out` must match the source frames in shape and dtype and live on %s" % out_device)
+    jobs, lanes = [], {}
+    for dev, (a, b) in zip(devices, shard_plan(int(src.shape[0]), len(devices))):
+        if b > a:
+            lane = lanes[dev] = lanes.get(dev, -1) + 1
+            jobs.append((dev, lane, a, b, make_fn(dev), torch.cuda.current_stream(dev)))
+    errors = [None] * len(jobs)
+
+    def work(k, dev, lane, a, b, fn, stream):
+        try:
+            with torch.cuda.device(dev), torch.cuda.stream(stream):
+                stream_frames(src[a:b], lambda f, i: fn(f, a + i), chunk, out_device, dev, out=out[a:b], lane=lane)
+        except BaseException as e:               # re-raised in the calling thread
+            errors[k] = e
+
+    threads = [threading.Thread(target=work, args=(k,) + job, name="vrgdg-shard-%d" % k) for k, job in enumerate(jobs)]
+    try:
+        for t in threads:
+            t.start()
+    finally:
+        for t in threads:
+            if t.ident is not None:
+                t.join()
+    for e in errors:
+        if e is not None:
+            raise e
     return out

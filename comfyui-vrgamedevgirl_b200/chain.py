@@ -11,39 +11,69 @@ import torch
 
 from . import _native as nv
 from . import ops
-from ._runtime import compute_device, stream_frames, upload
+from ._runtime import compute_device, cuda_device, stream_frames, stream_frames_sharded, upload
 
 
 class PostChain:
-    def __init__(self, grain=None, colormatch=None, lut=None, stencil=None, post_grain=None, device=None):
+    def __init__(self, grain=None, colormatch=None, lut=None, stencil=None, post_grain=None, device=None, devices=None):
         """
         grain / post_grain: dict(intensity, saturation_mix, seed, seed_mode=SEED_PER_CLIP)
         colormatch:         dict(reference_image=[1,H,W,3] tensor  |  ref_sums=[1,7] float64, strength)
         lut:                dict(lut_data={"lut","domain_min","domain_max"}, strength 0..10)
         stencil:            dict(op=STENCIL_*, strength, border=BORDER_REPLICATE)
+        devices:            CUDA devices run_host shards host batches over (default None: `device` alone).  The first one is `device`;
+                            a device may be listed twice (two workers on one card).
         """
-        self.device = torch.device(device) if device is not None else compute_device()
+        if devices is None:
+            self.device = torch.device(device) if device is not None else compute_device()
+            self.devices = [self.device]
+        else:
+            self.devices = [cuda_device(d) for d in devices]
+            if not self.devices:
+                raise ValueError("vrgdg_b200: PostChain(devices=...) needs at least one CUDA device")
+            if device is not None and cuda_device(device) != self.devices[0]:
+                raise ValueError("vrgdg_b200: PostChain(device=%s) is not the first of devices=%s" % (device, self.devices))
+            self.device = self.devices[0]
         self.grain, self.colormatch, self.lut, self.stencil, self.post_grain = grain, colormatch, lut, stencil, post_grain
-        self._lut_dev = None
-        self._ref_sums = None
+        # per device: the packed LUT and the reference statistics (made on `device`, copied to the others); per (device, worker on
+        # that device): the colour-match scratch
+        self._luts, self._refs, self._scratch = {}, {}, {}
         self.timing = None          # set to a list to collect (moments_start, moments_end, apply_start, apply_end) CUDA events per call
         # colour-match schedule (vrgdg_chain_cm_apply): one library call; `split` = the three-call path (statistics, parameters,
         # apply as separate entry points; what `timing` needs), `recompute` / `group_frames`: see include/vrgdg_b200.h
         self.split, self.recompute, self.group_frames, self.serial = False, False, 0, False
-        self._scratch = None
         if lut is not None:
-            self._lut_dev = ops.pack_lut(lut["lut_data"]["lut"], self.device)
+            packed = ops.pack_lut(lut["lut_data"]["lut"], self.device)
+            self._luts = {dev: packed if dev == self.device else ops.PackedLut(packed.data.to(dev), packed.size)
+                          for dev in dict.fromkeys(self.devices)}
         if colormatch is not None:
             self.set_reference(colormatch.get("reference_image"), colormatch.get("ref_sums"))
 
     # -- colour-match reference statistics (the only cross-rank quantity, see dist.py) --
     def set_reference(self, reference_image=None, ref_sums=None):
+        """The statistics are made once, on `device`, and copied to the other devices: a copy is bit-identical to a recomputation and
+        does not read the reference image once per GPU."""
         if ref_sums is not None:
-            self._ref_sums = ref_sums.to(self.device, torch.float64).reshape(-1, 7).contiguous()
+            sums = ref_sums.to(self.device, torch.float64).reshape(-1, 7).contiguous()
         elif reference_image is not None:
-            self._ref_sums = ops.lab_moments(upload(reference_image, self.device))
+            sums = ops.lab_moments(upload(reference_image, self.device))
         else:
             raise ValueError("colour match needs reference_image or ref_sums")
+        self._refs = {dev: sums if dev == self.device else sums.to(dev) for dev in dict.fromkeys(self.devices)}
+
+    @property
+    def _ref_sums(self):
+        """the reference statistics on `device`"""
+        return self._refs.get(self.device)
+
+    @staticmethod
+    def _on(table, dev):
+        """The copy in `table` for frames on `dev`.  A single-device chain has one copy, used whatever the frames' device."""
+        if len(table) == 1:
+            return next(iter(table.values()))
+        if dev not in table:
+            raise ValueError("vrgdg_b200: frames on %s, but this PostChain runs on %s" % (dev, list(table)))
+        return table[dev]
 
     def _desc(self, frames, first_frame, keep, ext_noise=None, fused_cm=False):
         d = nv.ChainDesc()
@@ -62,8 +92,9 @@ class PostChain:
                 dmin = data["domain_min"].to(dtype=fdt)
                 span = torch.clamp(data["domain_max"].to(dtype=fdt) - dmin, min=1e-6)
                 d.lut_enabled = 1
-                d.lut = self._lut_dev.data.data_ptr()
-                d.lut_size = self._lut_dev.size
+                packed = self._on(self._luts, frames.device)
+                d.lut = packed.data.data_ptr()
+                d.lut_size = packed.size
                 d.lut_dmin = (ctypes.c_float * 3)(*dmin.float().tolist())
                 d.lut_dspan = (ctypes.c_float * 3)(*span.float().tolist())
                 d.lut_blend, d.lut_one_minus_blend = blend, 1.0 - blend
@@ -89,7 +120,7 @@ class PostChain:
                 self._ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
                 self._ev[0].record()
             sums = ops.chain_lab_moments(frames, d, ext_noise=ext_noise)
-            params = ops.colormatch_params(sums, self._ref_sums)
+            params = ops.colormatch_params(sums, self._on(self._refs, frames.device))
             if self.timing is not None:
                 self._ev[1].record()
             keep.append(params)
@@ -102,11 +133,17 @@ class PostChain:
     def __call__(self, frames, first_frame=0, ext_noise=None, out=None, fast_math=False):
         """frames: CUDA [B,H,W,3]; first_frame: absolute index of frames[0] in the clip (keys the grain).
         ext_noise (tests): N(0,1) tensor replacing the generator; fast_math then selects the production arithmetic."""
+        return self._run(frames, first_frame, 0, ext_noise, out, fast_math)
+
+    def _run(self, frames, first_frame, worker, ext_noise=None, out=None, fast_math=False):
+        """__call__ with the colour-match scratch of `worker` (the index of a stream_frames_sharded worker on the frames' device)."""
         keep = []
         if self.colormatch is not None and not self.split and self.timing is None:
             d = self._desc(frames, first_frame, keep, ext_noise, fused_cm=True)
-            res, self._scratch = ops.chain_cm_apply(frames, d, self._ref_sums, ext_noise=ext_noise, out=out, fast_math=fast_math,
-                                                    recompute=self.recompute, group_frames=self.group_frames, scratch=self._scratch, serial=self.serial)
+            key = (frames.device, worker)
+            res, self._scratch[key] = ops.chain_cm_apply(frames, d, self._on(self._refs, frames.device), ext_noise=ext_noise, out=out,
+                                                         fast_math=fast_math, recompute=self.recompute, group_frames=self.group_frames,
+                                                         scratch=self._scratch.get(key), serial=self.serial)
             return res
         d = self._desc(frames, first_frame, keep, ext_noise)
         if self.timing is None:
@@ -123,7 +160,24 @@ class PostChain:
         self._ev = None
         return res
 
+    def make_fn(self, first_frame=0):
+        """make_fn of _runtime.stream_frames_sharded for this chain: every worker gets fn(frames, i) = self(frames, first_frame + i)
+        with a colour-match scratch of its own, so that two workers on one card never share one.  `first_frame`: absolute index of
+        the batch's first frame in the clip."""
+        if self.timing is not None:
+            raise ValueError("vrgdg_b200: PostChain.timing is collected by single-device calls only")
+        workers = {}
+
+        def make(dev):
+            k = workers[dev] = workers.get(dev, -1) + 1
+            return lambda f, i: self._run(f, first_frame + i, k)
+        return make
+
     def run_host(self, frames_cpu, chunk_frames=8, first_frame=0, out=None):
         """Host frames in, host frames out: chunked upload / compute / download on three streams.  Pass pinned tensors
-        (and a reusable pinned `out`) for asynchronous copies."""
-        return stream_frames(frames_cpu, lambda f, i: self(f, first_frame + i), chunk_frames, torch.device("cpu"), self.device, out=out)
+        (and a reusable pinned `out`) for asynchronous copies.  With several `devices` the batch is cut into one contiguous shard per
+        device, each streamed by its own host thread into its slice of one result (stream_frames_sharded); the result is
+        bit-identical to one device's."""
+        if len(self.devices) == 1:
+            return stream_frames(frames_cpu, lambda f, i: self(f, first_frame + i), chunk_frames, torch.device("cpu"), self.device, out=out)
+        return stream_frames_sharded(frames_cpu, self.make_fn(first_frame), chunk_frames, torch.device("cpu"), self.devices, out=out)

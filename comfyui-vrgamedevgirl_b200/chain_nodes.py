@@ -10,7 +10,7 @@
 import torch
 
 from . import _native as nv
-from ._runtime import compute_device, result_device, stream_frames, upload
+from ._runtime import compute_device, devices_from_env, result_device, stream_frames, stream_frames_sharded, upload
 from .chain import PostChain
 from .filter_nodes import _as_frames, draw_seed
 from .lut_nodes import NO_LUTS, VRGDG_LUTS, _list_lut_files
@@ -73,8 +73,13 @@ class VRGDG_B200_PostChain:
             stencil = dict(op=op, strength=float(sharpen_strength), border=nv.BORDER_ZERO if use_gpu else nv.BORDER_REPLICATE)
         if grain is None and cm is None and lut is None and stencil is None:
             return (images,)
-        chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, device=dev)
-        out = stream_frames(images, lambda f, i: chain(f, first_frame=i), batch_size, result_device(images), dev)
+        devs = devices_from_env() if images.device.type == "cpu" else None
+        if devs is None:
+            chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, device=dev)
+            out = stream_frames(images, lambda f, i: chain(f, first_frame=i), batch_size, result_device(images), dev)
+        else:                                    # host batch sharded over the VRGDG_DEVICES cards, bit-identical to one card
+            chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, devices=devs)
+            out = stream_frames_sharded(images, chain.make_fn(), batch_size, result_device(images), devs)
         return (out,)
 
 
@@ -110,14 +115,17 @@ class VRGDG_B200_EnhanceFrames:
             if float(grain_intensity) > 0 else None
         if stencil is None and post is None:
             return (images,)
+        devs = devices_from_env() if images.device.type == "cpu" else None
         if stencil is None:
             from . import ops
             s = post["saturation_mix"]
-            fn = lambda f, i: ops.grain(f, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start) + i, seed_mode=nv.SEED_PER_FRAME)
+            make_fn = lambda d: lambda f, i: ops.grain(f, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start) + i,
+                                                       seed_mode=nv.SEED_PER_FRAME)
         else:
-            chain = PostChain(stencil=stencil, post_grain=post, device=dev)
-            fn = lambda f, i: chain(f, first_frame=int(frame_start) + i)
-        return (stream_frames(images, fn, 8, result_device(images), dev),)
+            make_fn = PostChain(stencil=stencil, post_grain=post, device=None if devs else dev, devices=devs).make_fn(int(frame_start))
+        if devs is None:
+            return (stream_frames(images, make_fn(dev), 8, result_device(images), dev),)
+        return (stream_frames_sharded(images, make_fn, 8, result_device(images), devs),)   # host batch sharded over the VRGDG_DEVICES cards
 
 
 class VRGDG_B200_HistogramColorMatch:
