@@ -10,7 +10,7 @@ import threading
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("VRGDG_B200_LIB") or os.path.join(_HERE, "lib", "libvrgdg_b200.so")   # env override: build experiments only
+LIB_PATH = os.path.join(_HERE, "lib", "libvrgdg_b200.so")
 
 VRGDG_OK = 0
 E_INVALID, E_UNSUPPORTED, E_CUDA, E_ALIGN = -1, -2, -3, -4

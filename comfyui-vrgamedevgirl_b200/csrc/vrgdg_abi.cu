@@ -392,8 +392,7 @@ static int chain_point_params(const vrgdg_chain_desc* d, int B, int H, int W, Po
  * frames) and the grain + forward-Lab half of the colour match has already happened: stages become ST_CMF [| ST_LUT].
  * cm_params (when non-null) replaces desc->cm_params; frame_offset is added to both grain frame indices (group scheduling). */
 static int chain_apply_core(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* d,
-                            const void* ext_noise, bool fast, void* stream, const float* cm_params, bool from_f, int64_t frame_offset,
-                            int grid_limit = 0) {
+                            const void* ext_noise, bool fast, void* stream, const float* cm_params, bool from_f, int64_t frame_offset) {
   if (!d) return fail(VRGDG_E_INVALID, "vrgdg_chain_apply: null descriptor");
   int rc = check_frames(in, out, B, H, W, dtype, "vrgdg_chain_apply");
   if (rc) return rc;
@@ -405,7 +404,6 @@ static int chain_apply_core(const void* in, void* out, int B, int H, int W, int 
   if ((rc = get_ctx(stream, ctx))) return rc;
   TileParams Q;
   memset(&Q, 0, sizeof(Q));
-  Q.grid_limit = grid_limit;
   int mask = 0;
   bool exact = true;
   vrgdg_chain_desc dd = *d;
@@ -590,13 +588,6 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
   // registers) of group g+1 runs on a low-priority side stream WHILE the apply pass (L1 data-pipe bound, two resident tile CTAs per
   // SM that leave exactly that much of the register file) of group g runs on a high-priority one; f-planes and partials are double
   // buffered; events fork the side streams from the caller's stream and join them back, so the call stays stream-ordered.
-  // Tile CTAs of the apply pass while a statistics pass runs beside it: every tile CTA less frees registers for 3.5 more 128-thread
-  // statistics blocks.  Default 0 = no limit; VRGDG_PIPE_TILE_CTAS overrides (tuning only).
-  int tile_ctas = 0;
-  if (piped) {
-    const char* ev = getenv("VRGDG_PIPE_TILE_CTAS");
-    tile_ctas = ev ? atoi(ev) : 0;
-  }
   CmStreams* ss = nullptr;
   cudaEvent_t ev_start = nullptr, ev_p1[2] = {nullptr, nullptr}, ev_p2[2] = {nullptr, nullptr};
   LaunchCtx lo = ctx, hi = ctx;
@@ -651,7 +642,7 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
     }
     // pass 2: the fused apply, from the f-planes (no grain, no forward Lab) or from the frames
     rc = chain_apply_core(planes ? reinterpret_cast<const void*>(fplanes[buf]) : reinterpret_cast<const void*>(gin), gout, n, H, W, dtype, desc, gnoise, fast,
-                          piped ? reinterpret_cast<void*>(hi.stream) : stream, params + (int64_t)g0 * 12, planes, g0, piped ? tile_ctas : 0);
+                          piped ? reinterpret_cast<void*>(hi.stream) : stream, params + (int64_t)g0 * 12, planes, g0);
     if (rc) { cleanup(); return rc; }
     if (piped) {
       if ((e = cudaEventRecord(ev_p2[buf], hi.stream)) != cudaSuccess) { cleanup(); return fail_cuda(e, "vrgdg_chain_cm_apply (record)"); }

@@ -104,8 +104,7 @@ static cudaError_t launch_tile_k(const CUtensorMap* tmap, const void* in, void* 
   if (MASK & ST_LUT) cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)((smem + 1024) * TileCfg<T, MASK>::MINB * 100 / (228 * 1024)) + 1);
   static int occ = occupancy_of(kern, NT, smem);
   if (Q.total_tiles == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>(Q.total_tiles, (int64_t)ctx.sms * occ);
-  if (Q.grid_limit > 0 && grid > Q.grid_limit) grid = Q.grid_limit;
+  const int grid = (int)std::min<int64_t>(Q.total_tiles, (int64_t)ctx.sms * occ);
   CUtensorMap dummy;
   if (!tmap) { memset(&dummy, 0, sizeof(dummy)); tmap = &dummy; }
   kern<<<grid, NT, smem, ctx.stream>>>(*tmap, reinterpret_cast<const T*>(in), reinterpret_cast<T*>(out), Q);

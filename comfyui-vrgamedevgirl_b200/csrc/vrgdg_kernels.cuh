@@ -81,10 +81,6 @@ struct PointParams {
   LutParams lut;
 };
 
-#ifndef VRGDG_LUT_POLY
-#define VRGDG_LUT_POLY 1             // 0: the fast chains interpolate the corner cells too (A/B switch of tools/build_variant.sh)
-#endif
-
 // One pixel through the enabled stages; (zr,zg,zb) = this pixel's N(0,1) triple (generator or external).
 template <int MASK, bool EXACT>
 __device__ __forceinline__ void process_pixel(const PointParams& P, const CmFold& cmf, float zr, float zg, float zb,
@@ -101,7 +97,7 @@ __device__ __forceinline__ void process_pixel(const PointParams& P, const CmFold
   }
   if (MASK & ST_LUT) {
     float x0 = r, x1 = g, x2 = b;
-    if (EXACT || !VRGDG_LUT_POLY) lut3d_eval<EXACT>(P.lut, r, g, b);
+    if (EXACT) lut3d_eval<EXACT>(P.lut, r, g, b);
     else lutp_eval(P.lut, r, g, b);                  // fast arithmetic: polynomial cells, 7 FMAs per channel
     if (P.lut.blend < 1.0f) {
       r = lut_blend<EXACT>(x0, r, P.lut.blend, P.lut.one_minus_blend);
@@ -115,7 +111,7 @@ __device__ __forceinline__ void process_pixel(const PointParams& P, const CmFold
 // LANE_PAIR: the sector loads are split between lane pairs (lut_eval_lane_pair): every lane of a full warp must call it.
 template <bool EXACT, bool LANE_PAIR>
 __device__ __forceinline__ void lut_pair(const PointParams& P, float* p) {
-  constexpr bool POLY = !EXACT && VRGDG_LUT_POLY;
+  constexpr bool POLY = !EXACT;
   float x[6] = {p[0], p[1], p[2], p[3], p[4], p[5]};
   if (LANE_PAIR) lut_eval_lane_pair<POLY, EXACT>(P.lut, p, p + 3);
   else if (POLY) lutp_eval2(P.lut, p, p + 3);
@@ -333,7 +329,6 @@ struct TileParams {
   int exact_stencil;            // 1: reference evaluation order, one rounding per op (bit-exact NumPy-path results for fp32)
   int use_tma;                  // 0: cooperative bounds-checked loads (any alignment)
   int vec_store;                // rows 16-byte aligned -> 16-byte stores
-  int grid_limit;               // > 0: launch at most this many persistent CTAs (pipelined colour-match schedule leaves room for the statistics pass)
 };
 
 // HEAVY = the LUT gather runs in the pre-stage.  Two 256-thread CTAs per SM beat one 480-thread CTA on the fused grain + LUT + unsharp
@@ -352,47 +347,27 @@ template <typename T, int MASK> struct TileCfg {
   static constexpr int PADL = 16 / (int)sizeof(T);    // box starts 16 BYTES left of the tile: TMA needs a 16-byte aligned start address
   static constexpr int TXE = sizeof(T) == 1 ? 192 : 240;   // output elements per tile row: multiple of 6 and of VEC, TXE*sizeof(T) % 16 == 0 (every box start
                                                             // must be 16-byte aligned: an unaligned start is an illegal instruction), PADL + TXE + 3 <= BX
-#ifndef VRGDG_TILE_ROWS
-#define VRGDG_TILE_ROWS 32
-#endif
-  static constexpr int TY = VRGDG_TILE_ROWS;          // output rows per tile
+  static constexpr int TY = 32;                       // output rows per tile
   static constexpr int ROWS = TY + 2;
-#ifndef VRGDG_HEAVY_THREADS
-#define VRGDG_HEAVY_THREADS 256
-#endif
-  static constexpr int THREADS = HEAVY ? VRGDG_HEAVY_THREADS : 256;
+  static constexpr int THREADS = 256;
   // Register budget of the LUT configurations on fp32 frames: declaring a larger block than is ever launched lowers ptxas' register
   // cap (65536 / (LB_THREADS * MINB)) below the 128 that two 256-thread CTAs would allow, which leaves room in the register file for
   // the statistics blocks of the NEXT frame group next to two resident tile CTAs (pipelined colour-match schedule, vrgdg_abi.cu).
   // 256 (104-109 registers) fits one 128-thread statistics block beside two tile CTAs, 320 (91-94 registers) two, 352 (80 registers)
   // three or four.  At 80 registers the sm_90a LUT tile kernels spill 12-108 bytes per thread (ptxas -v).  352 was chosen by a sweep
   // on an earlier GPU with the same register file and shared memory per SM and has not been re-swept on H100.
-#ifndef VRGDG_HEAVY_LB
-#define VRGDG_HEAVY_LB 352
-#endif
-  static constexpr int LB_THREADS = (HEAVY && sizeof(T) == 4 && VRGDG_HEAVY_LB > THREADS) ? VRGDG_HEAVY_LB : THREADS;
-#ifndef VRGDG_HEAVY_MINB
-#define VRGDG_HEAVY_MINB 2
-#endif
-#ifndef VRGDG_HEAVY_NS
-#define VRGDG_HEAVY_NS (WORK ? 1 : 2)                 // in-place (fp32) tiles need the staged tile until the stencil is done
-#endif
-#ifndef VRGDG_LIGHT_MINB
-#define VRGDG_LIGHT_MINB 2
-#endif
-#ifndef VRGDG_LIGHT_NS
-#define VRGDG_LIGHT_NS 3
-#endif
+  static constexpr int LB_THREADS = (HEAVY && sizeof(T) == 4) ? 352 : THREADS;
   // plain stencils on 16-bit frames need few registers and 17 KB per staged tile: four CTAs per SM with a 2-stage ring
   // (fp32 tiles are 35 KB per stage and gain nothing from a third CTA)
   static constexpr bool SLIM = (MASK == 0) && (sizeof(T) == 2);
-  static constexpr int MINB = HEAVY ? VRGDG_HEAVY_MINB : (SLIM ? 4 : VRGDG_LIGHT_MINB);
+  static constexpr int MINB = SLIM ? 4 : 2;
   static constexpr int COLS = TXE / VEC;              // threads across
   static constexpr int RG = (THREADS / COLS) >= 8 ? 8 : 4;   // row groups: COLS*RG active threads
   static constexpr int RPT = TY / RG;                 // rows per thread
   static constexpr int PPR = TXE / 3 + 2;             // halo-tile pixels per row
   static constexpr int PAIRS = PPR / 2 + 1;           // generator pixel pairs covering them (tile x origin is even)
-  static constexpr int NS = HEAVY ? VRGDG_HEAVY_NS : ((GPLANE || SLIM) ? 2 : VRGDG_LIGHT_NS);   // pipeline stages
+  // pipeline stages; in-place (fp32) LUT tiles need the staged tile until the stencil is done, so they keep a second stage
+  static constexpr int NS = HEAVY ? (WORK ? 1 : 2) : ((GPLANE || SLIM) ? 2 : 3);
   static constexpr int STAGE_BYTES = ROWS * BX * (int)sizeof(T);
   static_assert(PADL + TXE + 3 <= BX, "box too narrow");
   static_assert(TY % RG == 0 && COLS * RG <= THREADS, "thread mapping");
@@ -685,14 +660,9 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
   // WORK configurations copy the staged tile into the fp32 work tile in the pre-stage, so the stage is free again as soon as
   // the pre-stage barrier has passed: its refill (tile k + NS) is issued there and overlaps the stencil phase; in-place
   // configurations refill at the top of the next iteration (tile k + NS - 1 into the stage the previous iteration used).
-#ifndef VRGDG_EARLY_REFILL
-#define VRGDG_EARLY_REFILL 1
-#endif
-  constexpr bool EARLY = WORK && (VRGDG_EARLY_REFILL != 0);
-  // a single in-place stage (NS == 1 without a work tile) is refilled at the END of the iteration, once the stencil has read it;
-  // the load latency is then covered by the other resident CTAs of the SM instead of a second stage
-  constexpr bool LATE1 = !EARLY && NS == 1;
-  constexpr uint32_t AHEAD = EARLY ? NS : (LATE1 ? 1 : NS - 1);
+  constexpr bool EARLY = WORK;
+  static_assert(WORK || NS >= 2, "an in-place tile is read until the stencil is done: refilling ahead needs a second stage");
+  constexpr uint32_t AHEAD = EARLY ? NS : NS - 1;
   if (tma && tid == 0) {
     for (uint32_t k = 0; k < AHEAD && k < n_my; ++k) issue(k);
   }
@@ -704,7 +674,7 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
     T* raw = reinterpret_cast<T*>(reinterpret_cast<uint8_t*>(stage0) + (size_t)s * C::STAGE_BYTES);
 
     if (tma) {
-      if (!EARLY && !LATE1 && tid == 0 && k + NS - 1 < n_my) {
+      if (!EARLY && tid == 0 && k + NS - 1 < n_my) {
         fence_proxy_async();          // order earlier generic-proxy accesses of that stage before the async write
         issue(k + NS - 1);
       }
@@ -832,7 +802,6 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
     }
     if (tma) fence_proxy_async();   // generic-proxy writes to this stage happen-before its next async refill
     __syncthreads();   // every thread is done with this stage before it is refilled
-    if (LATE1 && tma && tid == 0 && k + 1 < n_my) issue(k + 1);
   }
 }
 
@@ -867,11 +836,10 @@ __device__ __forceinline__ void moments_add(float& r, float& g, float& b, float*
 // ST_CMF second pass.
 // NT = 256 (two reduction units per block) or 128 (one: small enough to share an SM with two resident tile CTAs, see
 // vrgdg_chain_cm_apply's pipelined schedule).
-#ifndef VRGDG_MOMENT_SMALL_MINB
-#define VRGDG_MOMENT_SMALL_MINB 10     // 128-thread blocks per SM the register cap is computed for: 8 = 64 registers (three blocks fit beside two
-                                       // 80-register tile CTAs), 10 = 48 registers (four blocks; no spills on sm_90a; chosen on an earlier GPU, not re-swept on H100)
-#endif
-template <int NT> struct MomentLaunch { static constexpr int MINB = (NT == MOMENT_UNIT) ? VRGDG_MOMENT_SMALL_MINB : 4; };   // 256 threads: 64 registers as before
+// MINB = blocks per SM the register cap is computed for.  128 threads: 10 = 48 registers, so four blocks fit beside two 80-register
+// tile CTAs (8 = 64 registers would fit three); no spills on sm_90a; chosen on an earlier GPU, not re-swept on H100.  256 threads:
+// 4 = 64 registers.
+template <int NT> struct MomentLaunch { static constexpr int MINB = (NT == MOMENT_UNIT) ? 10 : 4; };
 template <typename T, bool GRAIN, bool VEC, int NT>
 __global__ void __launch_bounds__(NT, (MomentLaunch<NT>::MINB))
 k_lab_moments(const T* __restrict__ in, PointParams P, int row0, int rows, double* __restrict__ partials, float* __restrict__ fplanes) {
