@@ -307,3 +307,12 @@ def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None):
         if e is not None:
             raise e
     return out
+
+
+def run_frames(images, make_fn, chunk, out_device, device, devices):
+    """The frame loop of every node.  A host batch with a host result is sharded over `devices` (the node's devices_from_env(),
+    None = not sharded) by stream_frames_sharded; anything else is the single-device stream_frames(images, make_fn(device), ...).
+    make_fn(dev) -> fn(cuda_frames, absolute_first_frame) is called in the calling thread, once per non-empty shard."""
+    if devices is not None and images.device.type == "cpu" and torch.device(out_device).type == "cpu":
+        return stream_frames_sharded(images, make_fn, chunk, out_device, devices)
+    return stream_frames(images, make_fn(device), chunk, out_device, device)

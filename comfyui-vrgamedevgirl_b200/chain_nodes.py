@@ -10,7 +10,7 @@
 import torch
 
 from . import _native as nv
-from ._runtime import compute_device, devices_from_env, result_device, stream_frames, stream_frames_sharded, upload
+from ._runtime import compute_device, devices_from_env, result_device, run_frames, upload
 from .chain import PostChain
 from .filter_nodes import _as_frames, draw_seed
 from .lut_nodes import NO_LUTS, VRGDG_LUTS, _list_lut_files
@@ -74,13 +74,8 @@ class VRGDG_B200_PostChain:
         if grain is None and cm is None and lut is None and stencil is None:
             return (images,)
         devs = devices_from_env() if images.device.type == "cpu" else None
-        if devs is None:
-            chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, device=dev)
-            out = stream_frames(images, lambda f, i: chain(f, first_frame=i), batch_size, result_device(images), dev)
-        else:                                    # host batch sharded over the VRGDG_DEVICES cards, bit-identical to one card
-            chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, devices=devs)
-            out = stream_frames_sharded(images, chain.make_fn(), batch_size, result_device(images), devs)
-        return (out,)
+        chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, device=None if devs else dev, devices=devs)
+        return (run_frames(images, chain.make_fn(), batch_size, result_device(images), chain.device, devs),)
 
 
 class VRGDG_B200_EnhanceFrames:
@@ -123,9 +118,7 @@ class VRGDG_B200_EnhanceFrames:
                                                        seed_mode=nv.SEED_PER_FRAME)
         else:
             make_fn = PostChain(stencil=stencil, post_grain=post, device=None if devs else dev, devices=devs).make_fn(int(frame_start))
-        if devs is None:
-            return (stream_frames(images, make_fn(dev), 8, result_device(images), dev),)
-        return (stream_frames_sharded(images, make_fn, 8, result_device(images), devs),)   # host batch sharded over the VRGDG_DEVICES cards
+        return (run_frames(images, make_fn, 8, result_device(images), devs[0] if devs else dev, devs),)
 
 
 class VRGDG_B200_HistogramColorMatch:
@@ -160,10 +153,14 @@ class VRGDG_B200_HistogramColorMatch:
         with torch.cuda.device(dev):
             ref_counts = ops.hist_counts(upload(ref, dev).to(images.dtype))
 
-        def run(frames, first):
-            tables = ops.histmatch_tables(ops.hist_counts(frames), ref_counts)
-            return ops.histmatch_apply(frames, tables, t, 1.0 - t)
-        return (stream_frames(images, run, batch_size, result_device(images), dev),)
+        def make_fn(card):
+            counts = ref_counts.to(card)         # made once, copied to each card
+            def run(frames, first):
+                tables = ops.histmatch_tables(ops.hist_counts(frames), counts)
+                return ops.histmatch_apply(frames, tables, t, 1.0 - t)
+            return run
+        devs = devices_from_env() if images.device.type == "cpu" else None
+        return (run_frames(images, make_fn, batch_size, result_device(images), dev, devs),)
 
 
 class VRGDG_B200_TemporalSharpen:
@@ -194,12 +191,15 @@ class VRGDG_B200_TemporalSharpen:
             return (images,)
         s = float(strength)
 
-        def run(frames, first):          # the chunk's neighbours come from the clip itself (host or device tensor)
-            n = int(frames.shape[0])
-            prev = images[first - 1].to(dev) if first > 0 else None
-            nxt = images[first + n].to(dev) if first + n < T else None
-            return ops.temporal_sharpen(frames, s, prev, nxt)
-        return (stream_frames(images, run, batch_size, result_device(images), dev),)
+        def make_fn(card):
+            def run(frames, first):      # the chunk's neighbours come from the clip itself (host or device tensor), by absolute index
+                n = int(frames.shape[0])
+                prev = images[first - 1].to(card) if first > 0 else None
+                nxt = images[first + n].to(card) if first + n < T else None
+                return ops.temporal_sharpen(frames, s, prev, nxt)
+            return run
+        devs = devices_from_env() if images.device.type == "cpu" else None
+        return (run_frames(images, make_fn, batch_size, result_device(images), dev, devs),)
 
 
 class VRGDGVideoEnhanceRestoreOriginal:

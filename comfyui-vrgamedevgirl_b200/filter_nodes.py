@@ -10,7 +10,7 @@ import torch
 
 from . import _native as nv
 from . import ops
-from ._runtime import compute_device, result_device, stream_frames, upload
+from ._runtime import compute_device, devices_from_env, result_device, run_frames, upload
 
 _FLOATS = (torch.float32, torch.float16, torch.bfloat16)
 
@@ -56,7 +56,8 @@ class FastFilmGrain:
         # frame index, so the result does not depend on it (0 = whole batch, nodes.py:46)
         def run(frames, first):
             return ops.grain(frames, grain_intensity, sat, 1.0 - sat, seed, frame0=first, seed_mode=nv.SEED_PER_CLIP)
-        out = stream_frames(images, run, batch_size, result_device(images), compute_device(images))
+        devs = devices_from_env() if images.device.type == "cpu" else None
+        out = run_frames(images, lambda dev: run, batch_size, result_device(images), compute_device(images), devs)
         return (out,)
 
 
@@ -91,14 +92,21 @@ class ColorMatchToReference:
             ref_sums = ops.lab_moments(upload(reference_image, dev).to(images.dtype))
         d = nv.ChainDesc()
         d.colormatch_enabled, d.cm_t, d.cm_one_minus_t = 1, t, 1.0 - t
-        state = {"scratch": None}
-        def run(frames, first):
-            # one library call per chunk: statistics, parameters and the apply pass (which starts from the stored Lab f-planes for
-            # fp32 frames instead of repeating the forward transform)
-            rs = ref_sums if n_ref == 1 else ref_sums[first:first + frames.shape[0]]
-            out, state["scratch"] = ops.chain_cm_apply(frames, d, rs, scratch=state["scratch"])
-            return out
-        out = stream_frames(images, run, batch_size, result_device(images), dev)
+
+        def make_fn(card):
+            # the reference sums are made once and copied to each card; the scratch is the worker's own (two workers on one card
+            # must not share one)
+            sums = ref_sums.to(card)
+            state = {"scratch": None}
+            def run(frames, first):
+                # one library call per chunk: statistics, parameters and the apply pass (which starts from the stored Lab f-planes
+                # for fp32 frames instead of repeating the forward transform)
+                rs = sums if n_ref == 1 else sums[first:first + frames.shape[0]]
+                out, state["scratch"] = ops.chain_cm_apply(frames, d, rs, scratch=state["scratch"])
+                return out
+            return run
+        devs = devices_from_env() if images.device.type == "cpu" else None
+        out = run_frames(images, make_fn, batch_size, result_device(images), dev, devs)
         return (out,)
 
 
@@ -114,7 +122,8 @@ class _StencilNode:
         s = float(strength)
         def run(frames, first):
             return ops.stencil3x3(frames, op, s, border)
-        out = stream_frames(images, run, 8, result_device(images, numpy_path=not use_gpu), compute_device(images))
+        devs = devices_from_env() if images.device.type == "cpu" else None
+        out = run_frames(images, lambda dev: run, 8, result_device(images, numpy_path=not use_gpu), compute_device(images), devs)
         return (out,)
 
 

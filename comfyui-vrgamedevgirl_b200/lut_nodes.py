@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import ops
-from ._runtime import compute_device, stream_frames
+from ._runtime import compute_device, devices_from_env, run_frames
 
 LUTS_DIR = os.path.join(os.path.dirname(__file__), "LUTS")
 SUPPORTED_LUT_EXTENSIONS = (".cube",)
@@ -133,12 +133,16 @@ def _run_lut(image, lut_data, strength):
     dmin = lut_data["domain_min"].to(dtype=work.dtype)
     dmax = lut_data["domain_max"].to(dtype=work.dtype)
     span = torch.clamp(dmax - dmin, min=1e-6)
-    lut_dev = _device_lut(lut_data, dev)
     lo, sp = dmin.float().tolist(), span.float().tolist()
     if work.device.type == "cuda":
-        return ops.lut3d_apply(work.to(dev), lut_dev, lo, sp, blend, 1.0 - blend).to(device=image.device)
-    # host frames: the three-stream pipeline of the other nodes (chunked upload / lookup / download, pinned result)
-    return stream_frames(work, lambda f, i: ops.lut3d_apply(f, lut_dev, lo, sp, blend, 1.0 - blend), 0, image.device, dev)
+        return ops.lut3d_apply(work.to(dev), _device_lut(lut_data, dev), lo, sp, blend, 1.0 - blend).to(device=image.device)
+
+    # host frames: the three-stream pipeline of the other nodes (chunked upload / lookup / download, pinned result), sharded over the
+    # VRGDG_DEVICES cards.  make_fn runs in the calling thread, so the packed-table cache is never written from a worker.
+    def make_fn(card):
+        lut_dev = _device_lut(lut_data, card)
+        return lambda f, i: ops.lut3d_apply(f, lut_dev, lo, sp, blend, 1.0 - blend)
+    return run_frames(work, make_fn, 0, image.device, dev, devices_from_env())
 
 
 def _device_lut(lut_data, dev):
