@@ -9,7 +9,8 @@
 //   nearest : src = min(floor(dst * scale), in - 1)  (ATen "nearest", identity / exact-2x shortcuts give the same indices)
 //   bilinear: src = max(scale * (dst + 0.5) - 0.5, 0), two taps per axis
 //   bicubic : src = scale * (dst + 0.5) - 0.5, Keys kernel A = -0.75, four border-clamped taps per axis
-//   area    : adaptive average: rows floor(o*in/out) .. ceil((o+1)*in/out), summed in row-major order, then / rows / cols
+//   area    : adaptive average over [o*in / out, ((o+1)*in + out - 1) / out), i.e. floor(o*in/out) .. ceil((o+1)*in/out) in exact
+//             int64 arithmetic (ATen's start_index / end_index), summed in row-major order, then / rows / cols
 //
 // Nearest and area are bit-identical to torch; bilinear / bicubic agree to fp32 rounding (ATen picks between two differently
 // associated CPU kernels depending on the thread count, so "the" reference bit pattern is not defined; tests use 2e-6).
@@ -102,11 +103,11 @@ __global__ void __launch_bounds__(256) k_resize(const T* __restrict__ in, T* __r
 #pragma unroll
           for (int c = 0; c < 3; ++c) o[c] = fmaf(a[c], wy[j], o[c]);
         }
-      } else {   // area
-        const int xa = (int)floorf((float)((int64_t)rx * R.sw) / (float)R.rw);
-        const int xb = (int)ceilf((float)((int64_t)(rx + 1) * R.sw) / (float)R.rw);
-        const int ya = (int)floorf((float)((int64_t)ry * R.sh) / (float)R.rh);
-        const int yb = (int)ceilf((float)((int64_t)(ry + 1) * R.sh) / (float)R.rh);
+      } else {   // area: ATen's integer window bounds (an fp32 quotient rounds once o*in passes 2^24 and picks the wrong window)
+        const int xa = (int)(((int64_t)rx * R.sw) / R.rw);
+        const int xb = (int)(((int64_t)(rx + 1) * R.sw + R.rw - 1) / R.rw);
+        const int ya = (int)(((int64_t)ry * R.sh) / R.rh);
+        const int yb = (int)(((int64_t)(ry + 1) * R.sh + R.rh - 1) / R.rh);
         for (int yy = ya; yy < yb; ++yy) {
           const T* row = src + yy * rs;
           for (int xx = xa; xx < xb; ++xx) {
