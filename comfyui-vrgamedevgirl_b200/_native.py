@@ -103,6 +103,7 @@ SIGNATURES = {
     "vrgdg_grain": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _u64, _i64, _i, _vp, _vp]),
     "vrgdg_grain_noise": (_i, [_vp, _i, _i, _i, _u64, _i64, _i, _vp]),
     "vrgdg_stencil3x3": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp]),
+    "vrgdg_stencil3x3_ch": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "vrgdg_lab_moments_scratch_bytes": (_i64, [_i]),
     "vrgdg_lab_moments": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i64, _vp]),
     "vrgdg_colormatch_params": (_i, [_vp, _i, _vp, _i, _vp, _vp]),

@@ -128,9 +128,10 @@ void zero_point(PointParams& P, int B, int H, int W) {
   P.B = B; P.H = H; P.W = W; P.hw = (int64_t)H * W;
 }
 
-int run_tile(const void* in, void* out, int B, int H, int W, int dtype, TileParams& Q, int mask, bool exact, const LaunchCtx& ctx) {
+// channels 3: launch_tile (every stage mask); channels 4: launch_tile_rgba (plain stencil, mask 0)
+int run_tile(const void* in, void* out, int B, int H, int W, int channels, int dtype, TileParams& Q, int mask, bool exact, const LaunchCtx& ctx) {
   if (in == out) return fail(VRGDG_E_INVALID, "tile kernels cannot run in place (in == out)");
-  Q.B = B; Q.H = H; Q.W = W; Q.RW = 3 * W;
+  Q.B = B; Q.H = H; Q.W = W; Q.RW = channels * W;
   int bx = 0, by = 0;
 #define GEO(T) (tile_geometry<T>(H, Q.RW, Q.tiles_x, Q.tiles_y, bx, by), 0)
   (void)DISPATCH_DTYPE(dtype, GEO);
@@ -143,9 +144,16 @@ int run_tile(const void* in, void* out, int B, int H, int W, int dtype, TilePara
   const size_t es = elem_size(dtype);
   Q.vec_store = (((size_t)Q.RW * es) % 16 == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0) ? 1 : 0;
   t_tile_path = tma ? "tma" : "generic";
-#define TL(T) launch_tile<T>(tma ? &map : nullptr, in, out, Q, mask, exact, ctx)
-  cudaError_t e = DISPATCH_DTYPE(dtype, TL);
+  cudaError_t e;
+  if (channels == 4) {
+#define TL(T) launch_tile_rgba<T>(tma ? &map : nullptr, in, out, Q, ctx)
+    e = DISPATCH_DTYPE(dtype, TL);
 #undef TL
+  } else {
+#define TL(T) launch_tile<T>(tma ? &map : nullptr, in, out, Q, mask, exact, ctx)
+    e = DISPATCH_DTYPE(dtype, TL);
+#undef TL
+  }
   if (e != cudaSuccess) return fail_cuda(e, "k_tile launch");
   return VRGDG_OK;
 }
@@ -280,11 +288,19 @@ int vrgdg_grain_noise(float* out, int B, int H, int W, uint64_t seed, int64_t fr
   return VRGDG_OK;
 }
 
-int vrgdg_stencil3x3(const void* in, void* out, int B, int H, int W, int dtype, int op, float strength, int border, void* stream) {
-  int rc = check_frames(in, out, B, H, W, dtype, "vrgdg_stencil3x3");
+static int stencil3x3_impl(const void* in, void* out, int B, int H, int W, int channels, int dtype, int op, float strength, int border,
+                           void* stream, const char* who) {
+  if (channels != 3 && channels != 4) return fail(VRGDG_E_INVALID, "%s: channels must be 3 or 4, got %d", who, channels);
+  int rc = check_frames(in, out, B, H, W, dtype, who);
   if (rc) return rc;
-  if (op < VRGDG_STENCIL_BOX_UNSHARP || op > VRGDG_STENCIL_SOBEL_GPU) return fail(VRGDG_E_INVALID, "vrgdg_stencil3x3: bad op %d", op);
-  if (border != VRGDG_BORDER_REPLICATE && border != VRGDG_BORDER_ZERO) return fail(VRGDG_E_INVALID, "vrgdg_stencil3x3: bad border %d", border);
+  if (op < VRGDG_STENCIL_BOX_UNSHARP || op > VRGDG_STENCIL_SOBEL_GPU) return fail(VRGDG_E_INVALID, "%s: bad op %d", who, op);
+  if (border != VRGDG_BORDER_REPLICATE && border != VRGDG_BORDER_ZERO) return fail(VRGDG_E_INVALID, "%s: bad border %d", who, border);
+  if (channels == 4) {
+    if (dtype == VRGDG_U8BGR) return fail(VRGDG_E_UNSUPPORTED, "%s: 4-channel uint8 frames are not supported (the byte format is 3-channel BGR)", who);
+    if (op == VRGDG_STENCIL_LAPLACIAN_GPU || op == VRGDG_STENCIL_SOBEL_GPU)
+      return fail(VRGDG_E_UNSUPPORTED, "%s: op %d (a torch conv2d path) takes 3 channels, got 4", who, op);
+    if ((int64_t)4 * W >= ((int64_t)1 << 31)) return fail(VRGDG_E_UNSUPPORTED, "%s: rows of %d RGBA pixels exceed 2^31 elements", who, W);
+  }
   if ((int64_t)B * H * W == 0) return VRGDG_OK;
   LaunchCtx ctx;
   if ((rc = get_ctx(stream, ctx))) return rc;
@@ -293,7 +309,16 @@ int vrgdg_stencil3x3(const void* in, void* out, int B, int H, int W, int dtype, 
   zero_point(Q.P, B, H, W);
   Q.op = op; Q.strength = strength; Q.border = border;
   Q.exact_stencil = (dtype == VRGDG_F32 || dtype == VRGDG_U8BGR) ? 1 : 0;   // fp32 / byte frames: bit-identical to the NumPy nodes; 16-bit frames round once anyway
-  return run_tile(in, out, B, H, W, dtype, Q, 0, true, ctx);
+  return run_tile(in, out, B, H, W, channels, dtype, Q, 0, true, ctx);
+}
+
+int vrgdg_stencil3x3(const void* in, void* out, int B, int H, int W, int dtype, int op, float strength, int border, void* stream) {
+  return stencil3x3_impl(in, out, B, H, W, 3, dtype, op, strength, border, stream, "vrgdg_stencil3x3");
+}
+
+int vrgdg_stencil3x3_ch(const void* in, void* out, int B, int H, int W, int channels, int dtype, int op, float strength, int border,
+                        void* stream) {
+  return stencil3x3_impl(in, out, B, H, W, channels, dtype, op, strength, border, stream, "vrgdg_stencil3x3_ch");
 }
 
 int64_t vrgdg_lab_moments_scratch_bytes(int B) {
@@ -438,7 +463,7 @@ static int chain_apply_core(const void* in, void* out, int B, int H, int W, int 
   Q.pseed = dd.post_seed; Q.pframe0 = dd.post_frame0; Q.pseed_mode = dd.post_seed_mode;
   grain_make_key(Q.pseed, Q.pseed_mode, Q.pkey);
   if (Q.post_enabled && mask == 0) mask = ST_POST;    // pure stencil + post grain: one Philox call per pixel pair via the grain plane
-  return run_tile(in, out, B, H, W, dtype, Q, mask, exact, ctx);
+  return run_tile(in, out, B, H, W, 3, dtype, Q, mask, exact, ctx);
 }
 
 static int chain_apply_impl(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* d,

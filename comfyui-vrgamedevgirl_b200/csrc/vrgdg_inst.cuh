@@ -93,15 +93,15 @@ void tile_geometry(int H, int RW, int& tiles_x, int& tiles_y, int& box_x, int& b
   box_y = C::ROWS;
 }
 
-template <typename T, int MASK, bool EXACT>
+template <typename T, int MASK, bool EXACT, int CH = 3>
 static cudaError_t launch_tile_k(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q, const LaunchCtx& ctx) {
-  auto kern = k_tile<T, MASK, EXACT>;
-  constexpr size_t smem = tile_smem_bytes<T, MASK>();
+  auto kern = k_tile<T, MASK, EXACT, CH>;
+  constexpr size_t smem = tile_smem_bytes<T, MASK, CH>();
   // per device context, so set on every launch (single-process multi-GPU hosts)
   cudaError_t attr = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (attr != cudaSuccess) return attr;
-  constexpr int NT = TileCfg<T, MASK>::THREADS;
-  if (MASK & ST_LUT) cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)((smem + 1024) * TileCfg<T, MASK>::MINB * 100 / (228 * 1024)) + 1);
+  constexpr int NT = TileCfg<T, MASK, CH>::THREADS;
+  if (MASK & ST_LUT) cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)((smem + 1024) * TileCfg<T, MASK, CH>::MINB * 100 / (228 * 1024)) + 1);
   static int occ = occupancy_of(kern, NT, smem);
   if (Q.total_tiles == 0) return cudaSuccess;
   const int grid = (int)std::min<int64_t>(Q.total_tiles, (int64_t)ctx.sms * occ);
@@ -136,6 +136,27 @@ cudaError_t launch_tile(const CUtensorMap* tmap, const void* in, void* out, Tile
     default: return cudaErrorInvalidValue;
   }
 #undef VRGDG_TL
+}
+
+// plain 3x3 stencil on RGBA frames (Q.RW = 4*W), read interleaved as stored.  The NumPy-path ops only: the torch paths (ops 3 and 5)
+// convolve with groups=3 and reject 4 channels in the reference.  Exact arithmetic on fp32 frames, the fast variant on 16-bit ones,
+// as vrgdg_stencil3x3 does, so that every channel equals the 3-channel kernel's result bit for bit.  Byte frames are 3-channel BGR.
+template <typename T>
+cudaError_t launch_tile_rgba(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q, const LaunchCtx& ctx) {
+  if constexpr (sizeof(T) == 1) {
+    return cudaErrorInvalidValue;
+  } else {
+    switch (Q.op) {
+      case 1: case 2: case 4:
+        if constexpr (sizeof(T) == 4) {
+          if (Q.exact_stencil) return launch_tile_k<T, 0, true, 4>(tmap, in, out, Q, ctx);
+        } else {
+          if (!Q.exact_stencil) return launch_tile_k<T, 0, false, 4>(tmap, in, out, Q, ctx);
+        }
+        return cudaErrorInvalidValue;
+      default: return cudaErrorInvalidValue;
+    }
+  }
 }
 
 // ---- moments -------------------------------------------------------------------------------------
@@ -197,6 +218,7 @@ cudaError_t launch_u8_out(const void* in, uint8_t* out, int64_t npix, const Laun
   template cudaError_t launch_point<T>(const void*, void*, const PointParams&, int, bool, const LaunchCtx&);              \
   template cudaError_t launch_lut_rgba<T>(const void*, void*, int64_t, const LutParams&, const LaunchCtx&);               \
   template cudaError_t launch_tile<T>(const CUtensorMap*, const void*, void*, TileParams&, int, bool, const LaunchCtx&);  \
+  template cudaError_t launch_tile_rgba<T>(const CUtensorMap*, const void*, void*, TileParams&, const LaunchCtx&);        \
   template cudaError_t launch_moments<T>(const void*, const PointParams&, bool, int, int, double*, double*, const LaunchCtx&, float*, bool); \
   template cudaError_t launch_adjust<T>(const void*, void*, const AdjustParams&, int, float*, float*, const LaunchCtx&);              \
   template cudaError_t launch_resize<T>(const void*, void*, const ResizeParams&, const LaunchCtx&);                       \

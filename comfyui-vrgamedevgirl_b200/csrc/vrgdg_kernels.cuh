@@ -4,7 +4,8 @@
 //   k_point : streaming per-pixel chain  [grain][colour match][3D LUT]          (no neighbourhood)
 //   k_tile  : TMA-staged halo tiles      [grain][colour match][3D LUT] -> 3x3 stencil -> [post grain]
 // plus the LAB moment reduction and the uint8 wire-format codecs.
-// Data layout: frames [B][H][W][3] channel-fastest; a frame row is RW = 3*W contiguous elements.
+// Data layout: frames [B][H][W][3] channel-fastest; a frame row is RW = 3*W contiguous elements.  The plain stencil of k_tile also
+// reads RGBA frames [B][H][W][4] interleaved as they are stored (CH = 4: RW = 4*W, neighbours e±4); every other kernel is RGB.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -313,7 +314,7 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
 // pre-stages applied to the whole halo tile in shared memory, 3x3 stencil, optional post grain.
 // =====================================================================================================
 struct TileParams {
-  int B, H, W, RW;              // RW = 3*W elements per row
+  int B, H, W, RW;              // RW = CH*W elements per row
   int tiles_x, tiles_y;
   int64_t total_tiles;
   PointParams P;                // pre-stages
@@ -338,7 +339,11 @@ struct TileParams {
 // Everything else uses 256-thread CTAs, a 3-stage ring and 2 CTAs per SM.
 // WORK = 16-bit frames with pre-stages: their fp32 results live in a separate work tile, and a thread then produces
 // 4 elements per row (16-byte shared loads at a 16-byte lane stride are bank-conflict free; 32-byte strides are not).
-template <typename T, int MASK> struct TileCfg {
+// CH = channels per pixel: the stencil's neighbours are e±CH.  CH = 4 (RGBA) exists for the plain stencil on float frames only:
+// the pre-stages and the post grain work on RGB pixel pairs, and byte frames are the 3-channel BGR wire format.
+template <typename T, int MASK, int CH = 3> struct TileCfg {
+  static_assert(CH == 3 || (CH == 4 && MASK == 0 && sizeof(T) != 1), "4-channel tiles: plain stencil on fp32 / fp16 / bf16 frames");
+  static constexpr int NCH = CH;
   static constexpr bool HEAVY = (MASK & ST_LUT) != 0;
   static constexpr bool WORK = (sizeof(T) == 1) || (((MASK & ST_PRE) != 0) && (sizeof(T) != 4));   // uint8 frames always convert into the work tile
   static constexpr bool GPLANE = (MASK & ST_POST) != 0;   // grain of the post stage, one Philox call per pixel pair, kept in its own fp32 plane
@@ -369,13 +374,15 @@ template <typename T, int MASK> struct TileCfg {
   // pipeline stages; in-place (fp32) LUT tiles need the staged tile until the stencil is done, so they keep a second stage
   static constexpr int NS = HEAVY ? (WORK ? 1 : 2) : ((GPLANE || SLIM) ? 2 : 3);
   static constexpr int STAGE_BYTES = ROWS * BX * (int)sizeof(T);
-  static_assert(PADL + TXE + 3 <= BX, "box too narrow");
+  static_assert(PADL + TXE + CH <= BX, "box too narrow: the right halo pixel must lie inside the box");
+  static_assert(PADL >= CH, "the left halo pixel must lie inside the box's 16-byte left pad");
+  static_assert(TXE % CH == 0 && TXE % VEC == 0, "tiles start on a pixel and on a thread's output run");
   static_assert(TY % RG == 0 && COLS * RG <= THREADS, "thread mapping");
 };
 
-template <typename T, int MASK>
+template <typename T, int MASK, int CH = 3>
 constexpr size_t tile_smem_bytes() {
-  using C = TileCfg<T, MASK>;
+  using C = TileCfg<T, MASK, CH>;
   size_t s = (size_t)C::NS * C::STAGE_BYTES;
   if (C::WORK) s += (size_t)C::ROWS * C::BX * 4;      // fp32 work tile
   if (C::GPLANE) s += (size_t)C::ROWS * C::BX * 4;    // post-grain plane
@@ -385,7 +392,7 @@ constexpr size_t tile_smem_bytes() {
 // replicate-border fix-up of a staged tile (np.pad(mode="edge") on the stage's input)
 template <typename E, typename CFG>
 __device__ __forceinline__ void fix_border(E* tile, int y0, int x0e, int H, int RW) {
-  constexpr int BX = CFG::BX, ROWS = CFG::ROWS, PADL = CFG::PADL, TY = CFG::TY, TXE = CFG::TXE;
+  constexpr int BX = CFG::BX, ROWS = CFG::ROWS, PADL = CFG::PADL, TY = CFG::TY, TXE = CFG::TXE, CH = CFG::NCH;
   const int vr = H - y0;        // image rows from y0 to the bottom
   const int ve = RW - x0e;      // row elements from x0e to the right edge
   const bool top = (y0 == 0), bot = (vr <= TY), left = (x0e == 0), right = (ve <= TXE);
@@ -398,11 +405,11 @@ __device__ __forceinline__ void fix_border(E* tile, int y0, int x0e, int H, int 
   }
   __syncthreads();
   if (left || right) {
-    for (int i = threadIdx.x; i < ROWS * 3; i += blockDim.x) {
-      int r = i / 3, c = i - r * 3;
+    for (int i = threadIdx.x; i < ROWS * CH; i += blockDim.x) {
+      int r = i / CH, c = i - r * CH;
       E* row = tile + r * BX;
-      if (left) row[PADL - 3 + c] = row[PADL + c];
-      if (right) row[PADL + ve + c] = row[PADL + ve - 3 + c];
+      if (left) row[PADL - CH + c] = row[PADL + c];
+      if (right) row[PADL + ve + c] = row[PADL + ve - CH + c];
     }
   }
   __syncthreads();
@@ -417,9 +424,11 @@ __device__ __forceinline__ uint4 lds128(const void* p) {
   return v;
 }
 
-// window row: WN = VEC+6 floats starting at element (f0 - 3) of the tile row
-template <typename E, int VEC>
+// window row: WN = VEC+2*CH floats starting at element (f0 - CH) of the tile row.  The loads are the same for CH = 3 and 4: the
+// fp32 words cover [f0-4, f0+VEC+4), the 16-bit words [f0-8, f0+16) (VEC == 8)
+template <typename E, int VEC, int CH = 3>
 __device__ __forceinline__ void load_window(const E* rowp /* -> tile column PADL+f0 */, float* w) {
+  static_assert(CH == 3 || CH == 4, "window of one pixel either side");
   if (sizeof(E) == 4) {
     // floats [f0-4, f0+VEC+4): (VEC+8)/4 aligned 16-byte words
     constexpr int NV = (VEC + 8) / 4;
@@ -432,13 +441,13 @@ __device__ __forceinline__ void load_window(const E* rowp /* -> tile column PADL
       tmp[4 * i + 2] = __uint_as_float(q.z); tmp[4 * i + 3] = __uint_as_float(q.w);
     }
 #pragma unroll
-    for (int i = 0; i < VEC + 6; ++i) w[i] = tmp[i + 1];
+    for (int i = 0; i < VEC + 2 * CH; ++i) w[i] = tmp[i + 4 - CH];
   } else {
     // 16-bit elements [f0-8, f0+16): three aligned 16-byte words (VEC == 8)
     union { uint4 q[3]; E e[24]; } u;
     u.q[0] = lds128(rowp - 8); u.q[1] = lds128(rowp); u.q[2] = lds128(rowp + 8);
 #pragma unroll
-    for (int i = 0; i < VEC + 6; ++i) w[i] = Elem<E>::ld(u.e[i + 5]);
+    for (int i = 0; i < VEC + 2 * CH; ++i) w[i] = Elem<E>::ld(u.e[i + 8 - CH]);
   }
 }
 
@@ -497,12 +506,12 @@ __device__ __forceinline__ void store_elems(T* __restrict__ out, const TileParam
   }
 }
 
-template <typename T, int OP, int MASK, bool XS>
+template <typename T, int OP, int MASK, bool XS, int CH = 3>
 __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, const float* gplane, T* __restrict__ out,
                                              const TileParams& Q, int frame, int y0, int x0e) {
-  using C = TileCfg<T, MASK>;
+  using C = TileCfg<T, MASK, CH>;
   constexpr bool WORK = C::WORK;
-  constexpr int VEC = C::VEC, BX = C::BX, PADL = C::PADL, WN = VEC + 6;
+  constexpr int VEC = C::VEC, BX = C::BX, PADL = C::PADL, WN = VEC + 2 * CH;
   const int tid = threadIdx.x;
   if (tid >= C::COLS * C::RG) return;
   const int cx = tid % C::COLS, rg = tid / C::COLS;
@@ -510,8 +519,8 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
   const int ge0 = x0e + f0;                 // first output element in the row
   const int rbase = rg * C::RPT;            // first output row of this thread == smem row of its upper neighbour
   auto load_row = [&](int srow, float* dst) {
-    if constexpr (WORK) load_window<float, VEC>(work + srow * BX + PADL + f0, dst);
-    else load_window<T, VEC>(raw + srow * BX + PADL + f0, dst);
+    if constexpr (WORK) load_window<float, VEC, CH>(work + srow * BX + PADL + f0, dst);
+    else load_window<T, VEC, CH>(raw + srow * BX + PADL + f0, dst);
   };
   const GrainFrame pgf = grain_frame(Q.pseed, Q.pframe0, frame, Q.pseed_mode);
   if (OP == 1 && !XS) {
@@ -519,10 +528,10 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
     float h0[VEC], h1[VEC], c1[VEC], wr[WN];
     load_row(rbase, wr);
 #pragma unroll
-    for (int e = 0; e < VEC; ++e) h0[e] = (wr[e] + wr[e + 3]) + wr[e + 6];
+    for (int e = 0; e < VEC; ++e) h0[e] = (wr[e] + wr[e + CH]) + wr[e + 2 * CH];
     load_row(rbase + 1, wr);
 #pragma unroll
-    for (int e = 0; e < VEC; ++e) { h1[e] = (wr[e] + wr[e + 3]) + wr[e + 6]; c1[e] = wr[e + 3]; }
+    for (int e = 0; e < VEC; ++e) { h1[e] = (wr[e] + wr[e + CH]) + wr[e + 2 * CH]; c1[e] = wr[e + CH]; }
 #pragma unroll
     for (int j = 0; j < C::RPT; ++j) {
       load_row(rbase + j + 2, wr);
@@ -530,10 +539,10 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
       float o[VEC];
 #pragma unroll
       for (int e = 0; e < VEC; ++e) {
-        const float h2 = (wr[e] + wr[e + 3]) + wr[e + 6];
+        const float h2 = (wr[e] + wr[e + CH]) + wr[e + 2 * CH];
         const float blur = ((h0[e] + h1[e]) + h2) * 0.1111111111111111f;      // sum / 9.0 to within 1 ulp
         o[e] = clamp01(fmaf(Q.strength, c1[e] - blur, c1[e]));                 // img + s*(img - blur)
-        h0[e] = h1[e]; h1[e] = h2; c1[e] = wr[e + 3];
+        h0[e] = h1[e]; h1[e] = h2; c1[e] = wr[e + CH];
       }
       if constexpr (C::GPLANE) {
         const float4* gp = reinterpret_cast<const float4*>(gplane + (rbase + j + 1) * BX + PADL + f0);
@@ -557,8 +566,8 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
       float o[VEC];
 #pragma unroll
       for (int e = 0; e < VEC; ++e) {
-        float n[9] = {w[0][e], w[0][e + 3], w[0][e + 6], w[1][e], w[1][e + 3], w[1][e + 6],
-                      w[2][e], w[2][e + 3], w[2][e + 6]};
+        float n[9] = {w[0][e], w[0][e + CH], w[0][e + 2 * CH], w[1][e], w[1][e + CH], w[1][e + 2 * CH],
+                      w[2][e], w[2][e + CH], w[2][e + 2 * CH]};
         o[e] = XS ? stencil_epilogue_exact(OP, n, Q.strength) : stencil_epilogue(OP, n, Q.strength);
       }
       if constexpr (C::GPLANE) {
@@ -606,10 +615,12 @@ __device__ __forceinline__ void pair_store6(float* p, bool word0, const float* e
   q[2] = make_float2(e[4], e[5]);
 }
 
-template <typename T, int MASK, bool EXACT>
-__global__ void __launch_bounds__((TileCfg<T, MASK>::LB_THREADS), (TileCfg<T, MASK>::MINB))
+// CH = 4: RGBA frames, plain stencil only (MASK 0); EXACT then selects the stencil arithmetic (exact on fp32 frames, fast on 16-bit
+// ones: the rule of the 3-channel stencil) and Q.op is one of the NumPy-path ops 1, 2, 4 (launch_tile_rgba).
+template <typename T, int MASK, bool EXACT, int CH = 3>
+__global__ void __launch_bounds__((TileCfg<T, MASK, CH>::LB_THREADS), (TileCfg<T, MASK, CH>::MINB))
 k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __restrict__ out, TileParams Q) {
-  using C = TileCfg<T, MASK>;
+  using C = TileCfg<T, MASK, CH>;
   constexpr int NT = C::THREADS;
   constexpr int VEC = C::VEC, BX = C::BX, PADL = C::PADL, TXE = C::TXE, TY = C::TY, ROWS = C::ROWS;
   constexpr int NS = C::NS;
@@ -780,7 +791,13 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
     // ---- 3x3 stencil, sliding 3-row register window, VEC outputs per thread per row ----
     {
       const float* wt = WORK ? work : nullptr;
-      if (Q.exact_stencil) {   // uniform; one specialised row loop per epilogue and arithmetic variant
+      if constexpr (CH != 3) {
+        switch (Q.op) {
+          case 1: stencil_rows<T, 1, MASK, EXACT, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 2: stencil_rows<T, 2, MASK, EXACT, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          default: stencil_rows<T, 4, MASK, EXACT, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+        }
+      } else if (Q.exact_stencil) {   // uniform; one specialised row loop per epilogue and arithmetic variant
         switch (Q.op) {
           case 1: stencil_rows<T, 1, MASK, true>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
           case 2: stencil_rows<T, 2, MASK, true>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
@@ -1043,6 +1060,8 @@ template <typename T> cudaError_t launch_lut_rgba(const void* in, void* out, int
                                                   const LaunchCtx& ctx);
 template <typename T> cudaError_t launch_tile(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q, int mask,
                                               bool exact, const LaunchCtx& ctx);
+template <typename T> cudaError_t launch_tile_rgba(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q,
+                                                   const LaunchCtx& ctx);
 template <typename T> cudaError_t launch_moments(const void* in, const PointParams& P, bool grain, int row0, int rows,
                                                  double* sums, double* partials, const LaunchCtx& ctx, float* fplanes = nullptr,
                                                  bool small_blocks = false);

@@ -15,9 +15,9 @@ from ._runtime import compute_device, devices_from_env, result_device, run_frame
 _FLOATS = (torch.float32, torch.float16, torch.bfloat16)
 
 
-def _as_frames(images, name="images"):
-    if not isinstance(images, torch.Tensor) or images.ndim != 4 or images.shape[-1] != 3:
-        raise ValueError("%s must be an IMAGE tensor shaped [batch, height, width, 3]" % name)
+def _as_frames(images, name="images", channels=(3,)):
+    if not isinstance(images, torch.Tensor) or images.ndim != 4 or images.shape[-1] not in channels:
+        raise ValueError("%s must be an IMAGE tensor shaped [batch, height, width, %s]" % (name, " or ".join(map(str, channels))))
     if images.dtype not in _FLOATS:
         images = images.float()
     return images
@@ -115,9 +115,14 @@ class _StencilNode:
     OP_GPU = nv.STENCIL_NONE
 
     def _apply(self, images, strength, use_gpu):
-        images = _as_frames(images)
-        # use_gpu=False -> the numpy path's semantics (edge-replicated border); True -> the torch path's (zero padding).
+        # RGB or RGBA: the reference's NumPy paths pad H and W only and filter every channel, and its avg_pool2d unsharp is per
+        # channel too; its conv2d paths (Laplacian / Sobel with use_gpu) have groups=3 and reject 4 channels, so these do here.
+        images = _as_frames(images, channels=(3, 4))
         op = self.OP_GPU if use_gpu else self.OP_CPU
+        if images.shape[-1] == 4 and op in (nv.STENCIL_LAPLACIAN_GPU, nv.STENCIL_SOBEL_GPU):
+            raise ValueError("%s with use_gpu=True takes 3-channel images (the torch path convolves with groups=3), got 4 channels"
+                             % type(self).__name__)
+        # use_gpu=False -> the numpy path's semantics (edge-replicated border); True -> the torch path's (zero padding).
         border = nv.BORDER_ZERO if use_gpu else nv.BORDER_REPLICATE
         s = float(strength)
         def run(frames, first):

@@ -101,13 +101,17 @@ def grain_noise(B, H, W, seed, frame0=0, seed_mode=nv.SEED_PER_CLIP, device="cud
 
 
 def stencil3x3(images, op, strength, border=nv.BORDER_REPLICATE):
-    t = _frames(images)
+    """3x3 sharpener on [B,H,W,3|4] CUDA frames (vrgdg_stencil3x3_ch).  RGBA frames are filtered on every channel, alpha included, as
+    the reference's NumPy paths do; the torch-path ops (STENCIL_LAPLACIAN_GPU / STENCIL_SOBEL_GPU) and uint8 frames take 3 channels."""
+    t = nv.require_cuda(images, "images")
+    if t.ndim != 4 or t.shape[-1] not in (3, 4):
+        raise ValueError("vrgdg_b200: images must be shaped [batch, height, width, 3 or 4], got %s" % (tuple(t.shape),))
     out = torch.empty_like(t)
-    B, H, W, _ = t.shape
+    B, H, W, C = t.shape
     lib = nv.load_library()
     with torch.cuda.device(t.device):
-        nv.check(lib.vrgdg_stencil3x3(nv.ptr(t), nv.ptr(out), B, H, W, nv.DTYPE_CODE[t.dtype], int(op), _f32(strength), int(border),
-                                      nv.stream_ptr(t.device)))
+        nv.check(lib.vrgdg_stencil3x3_ch(nv.ptr(t), nv.ptr(out), B, H, W, C, nv.DTYPE_CODE[t.dtype], int(op), _f32(strength), int(border),
+                                         nv.stream_ptr(t.device)))
     return out
 
 

@@ -122,6 +122,14 @@ VRGDG_API int vrgdg_grain(const void* in, void* out, int B, int H, int W, int dt
  * aligned, generic tile loader otherwise (same arithmetic). */
 VRGDG_API int vrgdg_stencil3x3(const void* in, void* out, int B, int H, int W, int dtype,
                      int op, float strength, int border, void* stream);
+/* vrgdg_stencil3x3 on frames [B,H,W,channels].  channels 3 is vrgdg_stencil3x3.  channels 4 (RGBA IMAGE tensors, e.g. from
+ * ComfyUI's Join Image with Alpha) runs the stencil on every channel, alpha included, reading the pixels interleaved as stored:
+ * the reference's NumPy paths pad H and W only (nodes.py:182-209, :266-289, :357-384), so each channel's result equals the
+ * 3-channel result on that channel.  4 channels take VRGDG_STENCIL_BOX_UNSHARP, _LAPLACIAN_CPU and _SOBEL_CPU with either border
+ * and float frames; the torch paths _LAPLACIAN_GPU / _SOBEL_GPU (conv2d with groups=3 in the reference) and uint8 frames (3-channel
+ * BGR) return VRGDG_E_UNSUPPORTED, other channel counts VRGDG_E_INVALID. */
+VRGDG_API int vrgdg_stencil3x3_ch(const void* in, void* out, int B, int H, int W, int channels, int dtype,
+                        int op, float strength, int border, void* stream);
 
 /* ---- colour match (Reinhard LAB mean/std transfer) ---------------------------------------------
  * Replaces ColorMatchToReference.match_color (nodes.py:97-121) incl. kornia rgb_to_lab / lab_to_rgb.
