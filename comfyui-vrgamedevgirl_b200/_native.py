@@ -118,6 +118,7 @@ SIGNATURES = {
     "vrgdg_adjust": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.POINTER(AdjustDesc), _vp, _vp, _vp, _i64, _vp]),
     "vrgdg_resize": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ResizeDesc), _vp]),
     "vrgdg_blend": (_i, [_vp, _vp, _vp, _i64, _i, _f, _f, _vp]),
+    "vrgdg_restore_blend": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ResizeDesc), _f, _f, _vp]),
     "vrgdg_hist_counts": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "vrgdg_histmatch_tables": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "vrgdg_histmatch_apply": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _f, _f, _vp]),

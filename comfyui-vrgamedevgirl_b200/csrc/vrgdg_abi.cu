@@ -768,6 +768,44 @@ int vrgdg_blend(const void* a, const void* b, void* out, int64_t n, int dtype, f
   return VRGDG_OK;
 }
 
+int vrgdg_restore_blend(const void* enhanced, const void* originals, void* out, int B, int n_restored, int He, int We, int Ce, int H,
+                        int W, int Co, int dtype, const vrgdg_resize_desc* d, float w_orig, float w_restored, void* stream) {
+  if (!d) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: null descriptor");
+  if (!dtype_ok(dtype) || dtype == VRGDG_U8BGR) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: float dtype expected, got %d", dtype);
+  if (B < 0 || He < 0 || We < 0 || H < 0 || W < 0) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: negative shape");
+  if ((Ce != 3 && Ce != 4) || (Co != 3 && Co != 4))
+    return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: channels must be 3 or 4, got %d enhanced and %d original", Ce, Co);
+  if (n_restored < 0 || n_restored > B) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: n_restored %d outside [0, %d]", n_restored, B);
+  if (d->mode < VRGDG_RESIZE_NEAREST || d->mode > VRGDG_RESIZE_AREA) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: unknown mode %d", d->mode);
+  if (d->src_w < 1 || d->src_h < 1 || d->src_x0 < 0 || d->src_y0 < 0 || (int64_t)d->src_x0 + d->src_w > We ||
+      (int64_t)d->src_y0 + d->src_h > He)
+    return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: ROI %d,%d %dx%d outside %dx%d frames", d->src_x0, d->src_y0, d->src_w, d->src_h, We, He);
+  if (d->res_w < 1 || d->res_h < 1 || d->off_x > 0 || d->off_y > 0 || (int64_t)d->off_x + d->res_w < W || (int64_t)d->off_y + d->res_h < H)
+    return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: resampled %dx%d at %d,%d does not cover the %dx%d frames", d->res_w, d->res_h,
+                d->off_x, d->off_y, W, H);
+  if ((int64_t)B * H * W == 0) return VRGDG_OK;
+  if (!originals || !out || (n_restored > 0 && !enhanced)) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: null pointer");
+  if (originals == out || enhanced == out) return fail(VRGDG_E_INVALID, "vrgdg_restore_blend: in-place restoring is not supported");
+  if ((reinterpret_cast<uintptr_t>(originals) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(enhanced)) % elem_size(dtype))
+    return fail(VRGDG_E_ALIGN, "vrgdg_restore_blend: frame pointer not aligned to its element size");
+  LaunchCtx ctx;
+  int rc = get_ctx(stream, ctx);
+  if (rc) return rc;
+  RestoreParams P;
+  ResizeParams& R = P.R;
+  R.B = n_restored; R.Hs = He; R.Ws = We; R.Cs = Ce; R.Ht = H; R.Wt = W; R.mode = d->mode;
+  R.x0 = d->src_x0; R.y0 = d->src_y0; R.sw = d->src_w; R.sh = d->src_h; R.rw = d->res_w; R.rh = d->res_h;
+  R.ox = d->off_x; R.oy = d->off_y;
+  R.scale_x = (float)d->src_w / (float)d->res_w;
+  R.scale_y = (float)d->src_h / (float)d->res_h;
+  P.B = B; P.Co = Co; P.n_restored = n_restored; P.w_orig = w_orig; P.w_restored = w_restored;
+#define RB(T) launch_restore<T>(enhanced, originals, out, P, ctx)
+  cudaError_t e = (dtype == VRGDG_F32) ? RB(float) : ((dtype == VRGDG_F16) ? RB(__half) : RB(__nv_bfloat16));
+#undef RB
+  if (e != cudaSuccess) return fail_cuda(e, "vrgdg_restore_blend");
+  return VRGDG_OK;
+}
+
 /* ---- histogram / CDF colour transfer (labelled extension, see vrgdg_histmatch.cuh) ---- */
 int vrgdg_hist_counts(const void* in, int B, int H, int W, int dtype, int row0, int rows, uint32_t* counts, void* stream) {
   if (!dtype_ok(dtype)) return fail(VRGDG_E_INVALID, "vrgdg_hist_counts: unknown dtype %d", dtype);

@@ -223,6 +223,7 @@ cudaError_t launch_u8_out(const void* in, uint8_t* out, int64_t npix, const Laun
   template cudaError_t launch_adjust<T>(const void*, void*, const AdjustParams&, int, float*, float*, const LaunchCtx&);              \
   template cudaError_t launch_resize<T>(const void*, void*, const ResizeParams&, const LaunchCtx&);                       \
   template cudaError_t launch_blend<T>(const void*, const void*, void*, int64_t, float, float, const LaunchCtx&);         \
+  template cudaError_t launch_restore<T>(const void*, const void*, void*, const RestoreParams&, const LaunchCtx&);        \
   template cudaError_t launch_temporal<T>(const void*, void*, const TemporalParams&, const LaunchCtx&);                   \
   template cudaError_t launch_hist_counts<T>(const void*, int, int, int, int, int, uint32_t*, const LaunchCtx&);          \
   template cudaError_t launch_histmatch_apply<T>(const void*, void*, int, int64_t, const float2*, float, float, const LaunchCtx&); \

@@ -294,6 +294,32 @@ def blend(a, b, weight_a, weight_b):
     return out
 
 
+def restore_blend(enhanced, originals, mode, weight_orig, weight_restored, roi=None, n_restored=None):
+    """The restore node in one launch (vrgdg_restore_blend): roi=(x0, y0, w, h) of enhanced [Be,He,We,3|4] is resampled to the
+    originals' size, and for the first n_restored frames (default min(B, Be)) clamp(originals * weight_orig + restored * weight_restored,
+    0, 1) replaces their RGB; the rest of originals [B,H,W,3|4] (alpha, later frames) is clamped.  Equals resize -> blend -> clamp."""
+    te, to = nv.require_cuda(enhanced, "enhanced"), nv.require_cuda(originals, "originals")
+    if te.ndim != 4 or te.shape[-1] not in (3, 4) or to.ndim != 4 or to.shape[-1] not in (3, 4):
+        raise ValueError("vrgdg_b200: restore_blend expects frames [B,H,W,3|4], got %s and %s" % (tuple(te.shape), tuple(to.shape)))
+    if te.dtype != to.dtype or te.device != to.device:
+        raise ValueError("vrgdg_b200: restore_blend operands differ (%s on %s vs %s on %s)" % (te.dtype, te.device, to.dtype, to.device))
+    if to.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+        raise ValueError("vrgdg_b200: restore_blend needs float frames, got %s" % to.dtype)
+    Be, He, We, Ce = te.shape
+    B, H, W, Co = to.shape
+    n = min(B, Be) if n_restored is None else int(n_restored)
+    if not 0 <= n <= min(B, Be):
+        raise ValueError("vrgdg_b200: n_restored %d outside [0, %d]" % (n, min(B, Be)))
+    x0, y0, sw, sh = roi if roi is not None else (0, 0, We, He)
+    d = nv.ResizeDesc(RESIZE_MODES[mode], int(x0), int(y0), int(sw), int(sh), int(W), int(H), 0, 0)
+    out = torch.empty_like(to)
+    lib = nv.load_library()
+    with torch.cuda.device(to.device):
+        nv.check(lib.vrgdg_restore_blend(nv.ptr(te), nv.ptr(to), nv.ptr(out), B, n, He, We, Ce, H, W, Co, nv.DTYPE_CODE[to.dtype],
+                                         ctypes.byref(d), float(weight_orig), float(weight_restored), nv.stream_ptr(to.device)))
+    return out
+
+
 def hist_counts(images, row0=0, rows=None):
     """Per-frame, per-channel (R, G, B) 256-bin counts over rows [row0,row0+rows): int32 [B,3,256] (histogram colour match, a labelled
     extension: vrgdg_hist_counts).  Counts are exact, so row-sharded counts of one image add up to the whole image's."""

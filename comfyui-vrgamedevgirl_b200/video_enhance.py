@@ -2,12 +2,13 @@
 
 Reference: VRGDG_VideoEnhanceNodes.py (_interpolation :45-51, _resize_batch :54-86, _restore_batch :89-106, the restore blend of
 VRGDG_VideoEnhanceRestore :404-418).  F.interpolate + crop / F.pad + clamp become ONE launch (vrgdg_resize): the fit mode only
-changes the ROI, the resampled size and the placement offset handed to the kernel.  The LTX sampling between prepare and restore,
+changes the ROI, the resampled size and the placement offset handed to the kernel; the restore's resample, blend and clamp are
+one vrgdg_restore_blend launch per streamed chunk of originals.  The LTX sampling between prepare and restore,
 the context dict and the logging are the reference's control plane and stay out of scope.
 """
 
 from . import ops
-from ._runtime import compute_device, upload
+from ._runtime import compute_device, devices_from_env, run_frames, upload
 
 
 def _interpolation(mode):
@@ -49,27 +50,59 @@ def _resize_batch(images, target_width, target_height, fit_mode, resize_method, 
     return out.to(images.device)
 
 
-def _restore_batch(images, source_width, source_height, fit_mode, resize_method):
+def _restore_roi(work_w, work_h, source_width, source_height, fit_mode):
+    """(x0, y0, w, h) of the enhanced frame that _restore_batch resamples back to the source size (:89-106): the letterbox content,
+    or the whole frame for the other fit modes."""
     if fit_mode != "Fit with letterbox (preserve all)":
-        return _resize_batch(images, source_width, source_height, "Stretch to dimensions", resize_method)
-    work_h, work_w = int(images.shape[1]), int(images.shape[2])
+        return 0, 0, int(work_w), int(work_h)
     scale = min(work_w / source_width, work_h / source_height)
     content_w = min(work_w, max(1, int(round(source_width * scale))))
     content_h = min(work_h, max(1, int(round(source_height * scale))))
-    left, top = max(0, (work_w - content_w) // 2), max(0, (work_h - content_h) // 2)
-    return _resize_batch(images, source_width, source_height, "Stretch to dimensions", resize_method,
-                         _roi=(left, top, content_w, content_h))
+    return max(0, (work_w - content_w) // 2), max(0, (work_h - content_h) // 2), content_w, content_h
+
+
+def _restore_batch(images, source_width, source_height, fit_mode, resize_method):
+    if fit_mode != "Fit with letterbox (preserve all)":
+        return _resize_batch(images, source_width, source_height, "Stretch to dimensions", resize_method)
+    roi = _restore_roi(int(images.shape[2]), int(images.shape[1]), source_width, source_height, fit_mode)
+    return _resize_batch(images, source_width, source_height, "Stretch to dimensions", resize_method, _roi=roi)
 
 
 def restore_frames(originals, enhanced, source_width, source_height, fit_mode, resize_method, enhancement_strength):
     """Tensor part of VRGDG_VideoEnhanceRestore.restore (:404-418): resample the enhanced frames back to the source size and lerp
-    them over the originals; frames the sampler did not return keep the original (clamped)."""
-    dev = compute_device(originals)
-    orig = upload(originals, dev)
-    restored = _restore_batch(upload(enhanced, dev), source_width, source_height, fit_mode, resize_method).to(orig.dtype)
-    usable = min(int(orig.shape[0]), int(restored.shape[0]))
+    them over the originals; frames the sampler did not return keep the original (clamped).  The result has the originals' device,
+    dtype and shape.
+
+    The originals stream through run_frames like every other frame node's IMAGE (host batches in VRGDG_STREAM_CHUNK_BYTES chunks,
+    sharded over VRGDG_DEVICES when the result is a host tensor too); each chunk uploads only the enhanced frames of the same
+    absolute indices and makes one vrgdg_restore_blend launch, so device memory follows the chunk, not the clip.  Enhanced frames of
+    another dtype than the originals take resize -> .to(dtype) -> blend per chunk: rounding the resample in the enhanced dtype
+    first is part of that result."""
+    if enhanced.ndim != 4 or enhanced.shape[0] < 1:
+        raise ValueError("Video Enhance requires a non-empty IMAGE batch.")
+    usable = min(int(originals.shape[0]), int(enhanced.shape[0]))
+    H, W = int(source_height), int(source_width)
+    if usable > 0 and (int(originals.shape[1]), int(originals.shape[2])) != (H, W):
+        raise ValueError("Video Enhance: the context's source size %dx%d differs from the original frames' %dx%d"
+                         % (W, H, int(originals.shape[2]), int(originals.shape[1])))
+    roi = _restore_roi(int(enhanced.shape[2]), int(enhanced.shape[1]), source_width, source_height, fit_mode)
+    mode = _interpolation(resize_method)
     strength = float(enhancement_strength)
-    output = orig.clamp(0, 1)
-    if usable > 0:
-        output[:usable, ..., :3] = ops.blend(orig[:usable, ..., :3], restored[:usable], 1.0 - strength, strength)
-    return output.to(originals.device)
+    fused = enhanced.dtype == originals.dtype and int(originals.shape[-1]) in (3, 4)
+
+    def make_fn(card):
+        def fn(orig, first):
+            n = max(0, min(first + int(orig.shape[0]), usable) - first)
+            enh = upload(enhanced[first:first + n], card)              # the same absolute frames; empty past the last one
+            if fused:
+                return ops.restore_blend(enh, orig, mode, 1.0 - strength, strength, roi=roi, n_restored=n)
+            out = orig.clamp(0, 1)
+            if n > 0:
+                restored = ops.resize(enh, H, W, mode, roi=roi).to(orig.dtype)
+                out[:n, ..., :3] = ops.blend(orig[:n, ..., :3], restored, 1.0 - strength, strength)
+            return out
+        return fn
+
+    dev = compute_device(originals)
+    devs = devices_from_env() if originals.device.type == "cpu" else None
+    return run_frames(originals, make_fn, 0, originals.device, dev, devs)

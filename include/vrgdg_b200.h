@@ -268,6 +268,16 @@ VRGDG_API int vrgdg_resize(const void* in, void* out, int B, int Hs, int Ws, int
  * originals * (1 - strength) + restored * strength (VRGDG_VideoEnhanceNodes.py:408-414).  n = elements. */
 VRGDG_API int vrgdg_blend(const void* a, const void* b, void* out, int64_t n, int dtype, float weight_a, float weight_b,
                 void* stream);
+/* The restore node's resample and blend in one pass (VRGDG_VideoEnhanceNodes.py:404-418).  originals and out are [B,H,W,Co],
+ * enhanced is [n_restored,He,We,Ce], all of one float dtype; Co and Ce are 3 or 4 and the enhanced alpha is ignored.  For frame
+ * b < n_restored and channel c < 3:
+ *   r   = dtype(clamp(resample(enhanced[b])[y][x][c], 0, 1))      exactly vrgdg_resize's output pixel for the same desc
+ *   out = dtype(clamp(originals * w_orig + r * w_restored, 0, 1))  exactly vrgdg_blend's, one rounding per operation
+ * Every other element (the alpha of 4-channel originals, frames b >= n_restored) is dtype(clamp(originals, 0, 1)), NaN kept.
+ * The resampled image must cover the output (off_x, off_y <= 0, off + res >= W, H) and the ROI must lie inside He x We.
+ * enhanced may be NULL when n_restored == 0; out must not alias either input.  B == 0 is a no-op. */
+VRGDG_API int vrgdg_restore_blend(const void* enhanced, const void* originals, void* out, int B, int n_restored, int He, int We, int Ce,
+                int H, int W, int Co, int dtype, const vrgdg_resize_desc* desc, float w_orig, float w_restored, void* stream);
 
 /* ---- histogram / CDF colour transfer — LABELLED EXTENSION, no reference counterpart ---------------------------------------------
  * BASELINE.json's north_star and configs[2] describe colour match as a "two-pass per-channel histogram + monotone-CDF LUT mapping";
