@@ -109,6 +109,7 @@ SIGNATURES = {
     "vrgdg_colormatch_params": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "vrgdg_colormatch_apply": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _f, _f, _vp]),
     "vrgdg_chain_apply": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp]),
+    "vrgdg_chain_apply_ch": (_i, [_vp, _vp, _i, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp]),
     "vrgdg_chain_apply_ext": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp, _i, _vp]),
     "vrgdg_chain_lab_moments": (_i, [_vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp, _vp, _i64, _vp]),
     "vrgdg_chain_lab_moments_ext": (_i, [_vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp, _vp, _vp, _i64, _vp]),

@@ -4,6 +4,7 @@ Semantics = the reference nodes applied one after another (FastFilmGrain nodes.p
 ColorMatchToReference :91-124 -> VRGDG_LUTS VRGDG_IV_Adjustments.py:345-361 -> FastUnsharpSharpen nodes.py:156-209),
 or the standalone enhancer's unsharp -> seeded grain (_apply_effects_batch,
 VRGDG_StandaloneVideoEnhancerNodes.py:278-294) via `post_grain`.  Any subset of stages may be enabled.
+RGBA frames take the subset the reference defines on 4 channels: LUT -> NumPy-path stencil (PostChain.check_frames).
 """
 import ctypes
 
@@ -130,13 +131,28 @@ class PostChain:
             d.cm_t, d.cm_one_minus_t = t, 1.0 - t
         return d
 
+    def check_frames(self, frames):
+        """RGBA frames [B,H,W,4] take the stages the reference defines on 4 channels: `lut` (RGB graded, alpha carried) and the
+        NumPy-path `stencil` ops (every channel filtered).  Anything else on RGBA raises ValueError here, before any device work."""
+        if not (isinstance(frames, torch.Tensor) and frames.ndim == 4 and frames.shape[-1] == 4):
+            return
+        for name in ("grain", "colormatch", "post_grain"):
+            if getattr(self, name) is not None:
+                raise ValueError("vrgdg_b200: PostChain stage `%s` takes 3-channel frames, got 4 channels (RGBA frames take `lut` and "
+                                 "`stencil` only)" % name)
+        if self.stencil is not None and self.stencil["op"] in (nv.STENCIL_LAPLACIAN_GPU, nv.STENCIL_SOBEL_GPU):
+            raise ValueError("vrgdg_b200: PostChain stencil op %d (a torch conv2d path) takes 3-channel frames, got 4 channels"
+                             % self.stencil["op"])
+
     def __call__(self, frames, first_frame=0, ext_noise=None, out=None, fast_math=False):
-        """frames: CUDA [B,H,W,3]; first_frame: absolute index of frames[0] in the clip (keys the grain).
-        ext_noise (tests): N(0,1) tensor replacing the generator; fast_math then selects the production arithmetic."""
+        """frames: CUDA [B,H,W,3], or [B,H,W,4] with only `lut` / `stencil` set (check_frames); first_frame: absolute index of
+        frames[0] in the clip (keys the grain).  ext_noise (tests): N(0,1) tensor replacing the generator; fast_math then selects the
+        production arithmetic."""
         return self._run(frames, first_frame, 0, ext_noise, out, fast_math)
 
     def _run(self, frames, first_frame, worker, ext_noise=None, out=None, fast_math=False):
         """__call__ with the colour-match scratch of `worker` (the index of a stream_frames_sharded worker on the frames' device)."""
+        self.check_frames(frames)
         keep = []
         if self.colormatch is not None and not self.split and self.timing is None:
             d = self._desc(frames, first_frame, keep, ext_noise, fused_cm=True)
@@ -178,6 +194,7 @@ class PostChain:
         (and a reusable pinned `out`) for asynchronous copies.  With several `devices` the batch is cut into one contiguous shard per
         device, each streamed by its own host thread into its slice of one result (stream_frames_sharded); the result is
         bit-identical to one device's."""
+        self.check_frames(frames_cpu)
         if len(self.devices) == 1:
             return stream_frames(frames_cpu, lambda f, i: self(f, first_frame + i), chunk_frames, torch.device("cpu"), self.device, out=out)
         return stream_frames_sharded(frames_cpu, self.make_fn(first_frame), chunk_frames, torch.device("cpu"), self.devices, out=out)

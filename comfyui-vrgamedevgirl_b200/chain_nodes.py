@@ -28,7 +28,9 @@ _SHARPENERS = {
 
 class VRGDG_B200_PostChain:
     """grain -> [colour match] -> 3D LUT -> sharpen in one pass over HBM (chain.PostChain).  Stage semantics and widget ranges
-    are those of the four reference nodes (nodes.py:20-34, :72-84, :135-147; VRGDG_IV_Adjustments.py:145-157)."""
+    are those of the four reference nodes (nodes.py:20-34, :72-84, :135-147; VRGDG_IV_Adjustments.py:145-157).  RGBA batches take
+    the LUT and the sharpeners the reference runs on 4 channels: grain_intensity 0, no reference_image, and use_gpu=False for
+    laplacian / sobel."""
 
     @classmethod
     def INPUT_TYPES(cls):
@@ -55,7 +57,17 @@ class VRGDG_B200_PostChain:
 
     def apply_chain(self, images, grain_intensity, saturation_mix, match_strength, lut_name, lut_strength, sharpen, sharpen_strength, use_gpu,
                     batch_size, reference_image=None):
-        images = _as_frames(images)
+        images = _as_frames(images, channels=(3, 4))
+        if images.shape[-1] == 4:
+            # RGBA: the stages the reference runs on 4 channels, VRGDG_LUTS and the NumPy-path sharpeners (the grain's gray
+            # broadcast, kornia's colour conversion and the torch-path conv2d with groups=3 raise there)
+            if float(grain_intensity) > 0:
+                raise ValueError("VRGDG_B200_PostChain: grain_intensity must be 0 for RGBA images (film grain takes 3 channels), got 4 channels")
+            if reference_image is not None:
+                raise ValueError("VRGDG_B200_PostChain: reference_image (colour match) takes 3-channel images, got 4 channels; disconnect it")
+            if use_gpu and _SHARPENERS[sharpen][1] in (nv.STENCIL_LAPLACIAN_GPU, nv.STENCIL_SOBEL_GPU):
+                raise ValueError("VRGDG_B200_PostChain: sharpen=%s with use_gpu=True takes 3-channel images (the torch path convolves "
+                                 "with groups=3), got 4 channels" % sharpen)
         dev = compute_device(images)
         grain = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), seed=draw_seed()) if float(grain_intensity) > 0 else None
         cm = None

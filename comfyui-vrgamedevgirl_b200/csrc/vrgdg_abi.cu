@@ -128,7 +128,7 @@ void zero_point(PointParams& P, int B, int H, int W) {
   P.B = B; P.H = H; P.W = W; P.hw = (int64_t)H * W;
 }
 
-// channels 3: launch_tile (every stage mask); channels 4: launch_tile_rgba (plain stencil, mask 0)
+// channels 3: launch_tile (every stage mask); channels 4: launch_tile_rgba (plain stencil, mask 0) or launch_tile_rgba_lut (mask ST_LUT)
 int run_tile(const void* in, void* out, int B, int H, int W, int channels, int dtype, TileParams& Q, int mask, bool exact, const LaunchCtx& ctx) {
   if (in == out) return fail(VRGDG_E_INVALID, "tile kernels cannot run in place (in == out)");
   Q.B = B; Q.H = H; Q.W = W; Q.RW = channels * W;
@@ -145,7 +145,11 @@ int run_tile(const void* in, void* out, int B, int H, int W, int channels, int d
   Q.vec_store = (((size_t)Q.RW * es) % 16 == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0) ? 1 : 0;
   t_tile_path = tma ? "tma" : "generic";
   cudaError_t e;
-  if (channels == 4) {
+  if (channels == 4 && mask == ST_LUT) {
+#define TL(T) launch_tile_rgba_lut<T>(tma ? &map : nullptr, in, out, Q, ctx)
+    e = DISPATCH_DTYPE(dtype, TL);
+#undef TL
+  } else if (channels == 4) {
 #define TL(T) launch_tile_rgba<T>(tma ? &map : nullptr, in, out, Q, ctx)
     e = DISPATCH_DTYPE(dtype, TL);
 #undef TL
@@ -480,6 +484,56 @@ int vrgdg_chain_apply(const void* in, void* out, int B, int H, int W, int dtype,
 int vrgdg_chain_apply_ext(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc,
                           const void* ext_noise, int flags, void* stream) {
   return chain_apply_impl(in, out, B, H, W, dtype, desc, ext_noise, (flags & VRGDG_CHAIN_FAST_MATH) != 0, stream);
+}
+
+/* RGBA frames through the stages the reference defines on 4 channels: the 3D LUT (RGB graded, alpha carried) and the NumPy-path
+ * stencils (every channel filtered).  Every argument is checked before the first CUDA call. */
+static int chain_apply_rgba(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* d, void* stream) {
+  const char* who = "vrgdg_chain_apply_ch";
+  if (!d) return fail(VRGDG_E_INVALID, "%s: null descriptor", who);
+  int rc = check_frames(in, out, B, H, W, dtype, who);
+  if (rc) return rc;
+  if (dtype == VRGDG_U8BGR) return fail(VRGDG_E_UNSUPPORTED, "%s: 4-channel uint8 frames are not supported (the byte format is 3-channel BGR)", who);
+  if (d->grain_enabled) return fail(VRGDG_E_UNSUPPORTED, "%s: the film grain stage takes 3 channels, got 4", who);
+  if (d->colormatch_enabled) return fail(VRGDG_E_UNSUPPORTED, "%s: the colour match stage takes 3 channels, got 4", who);
+  if (d->post_grain_enabled) return fail(VRGDG_E_UNSUPPORTED, "%s: the post grain stage takes 3 channels, got 4", who);
+  if (d->stencil_op < VRGDG_STENCIL_NONE || d->stencil_op > VRGDG_STENCIL_SOBEL_GPU) return fail(VRGDG_E_INVALID, "%s: bad stencil op %d", who, d->stencil_op);
+  if (d->stencil_border != VRGDG_BORDER_REPLICATE && d->stencil_border != VRGDG_BORDER_ZERO) return fail(VRGDG_E_INVALID, "%s: bad border %d", who, d->stencil_border);
+  if (d->stencil_op == VRGDG_STENCIL_LAPLACIAN_GPU || d->stencil_op == VRGDG_STENCIL_SOBEL_GPU)
+    return fail(VRGDG_E_UNSUPPORTED, "%s: stencil op %d (a torch conv2d path) takes 3 channels, got 4", who, d->stencil_op);
+  if ((int64_t)4 * W >= ((int64_t)1 << 31)) return fail(VRGDG_E_UNSUPPORTED, "%s: rows of %d RGBA pixels exceed 2^31 elements", who, W);
+  TileParams Q;
+  memset(&Q, 0, sizeof(Q));
+  int mask = 0;
+  bool exact = true;
+  if ((rc = chain_point_params(d, B, H, W, Q.P, mask, exact, nullptr, false))) return rc;   // the LUT stage (grain is refused above)
+  const bool stencil = d->stencil_op != VRGDG_STENCIL_NONE;
+  if ((int64_t)B * H * W == 0) return VRGDG_OK;
+  if (stencil && in == out) return fail(VRGDG_E_INVALID, "%s: the stencil cannot run in place (in == out)", who);
+  LaunchCtx ctx;
+  if ((rc = get_ctx(stream, ctx))) return rc;
+  if (!stencil) {
+    cudaError_t e = cudaSuccess;
+    if (mask == 0) {   // nothing enabled: copy
+      if (in != out) e = cudaMemcpyAsync(out, in, (size_t)B * H * W * 4 * elem_size(dtype), cudaMemcpyDeviceToDevice, ctx.stream);
+    } else {
+#define LR(T) launch_lut_rgba<T>(in, out, (int64_t)B * H * W, Q.P.lut, ctx)
+      e = DISPATCH_DTYPE(dtype, LR);
+#undef LR
+    }
+    if (e != cudaSuccess) return fail_cuda(e, who);
+    return VRGDG_OK;
+  }
+  Q.op = d->stencil_op; Q.strength = d->stencil_strength; Q.border = d->stencil_border;
+  Q.exact_stencil = dtype == VRGDG_F32 ? 1 : 0;   // the 3-channel chain's rule: bit-identical to the NumPy nodes on fp32 frames
+  return run_tile(in, out, B, H, W, 4, dtype, Q, mask, exact, ctx);
+}
+
+int vrgdg_chain_apply_ch(const void* in, void* out, int B, int H, int W, int channels, int dtype, const vrgdg_chain_desc* desc,
+                         void* stream) {
+  if (channels == 3) return vrgdg_chain_apply(in, out, B, H, W, dtype, desc, stream);
+  if (channels != 4) return fail(VRGDG_E_INVALID, "vrgdg_chain_apply_ch: channels must be 3 or 4, got %d", channels);
+  return chain_apply_rgba(in, out, B, H, W, dtype, desc, stream);
 }
 
 static int chain_moments_impl(const void* in, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc, const void* ext_noise,

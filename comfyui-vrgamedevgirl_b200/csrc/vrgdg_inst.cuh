@@ -159,6 +159,28 @@ cudaError_t launch_tile_rgba(const CUtensorMap* tmap, const void* in, void* out,
   }
 }
 
+// 3D LUT then 3x3 stencil on RGBA frames in one tile pass (Q.RW = 4*W, Q.P.lut filled): RGB graded, alpha carried as k_lut_rgba
+// carries it, every channel then filtered.  The LUT is the exact one of the 3-channel chain (no grain draws noise here); the stencil
+// arithmetic follows launch_tile_rgba's rule, exact on fp32 frames and fast on 16-bit ones, so that the RGB channels equal the
+// 3-channel fused chain's bit for bit.  NumPy-path ops only; byte frames are 3-channel BGR.
+template <typename T>
+cudaError_t launch_tile_rgba_lut(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q, const LaunchCtx& ctx) {
+  if constexpr (sizeof(T) == 1) {
+    return cudaErrorInvalidValue;
+  } else {
+    switch (Q.op) {
+      case 1: case 2: case 4:
+        if constexpr (sizeof(T) == 4) {
+          if (Q.exact_stencil) return launch_tile_k<T, ST_LUT, true, 4>(tmap, in, out, Q, ctx);
+        } else {
+          if (!Q.exact_stencil) return launch_tile_k<T, ST_LUT, true, 4>(tmap, in, out, Q, ctx);
+        }
+        return cudaErrorInvalidValue;
+      default: return cudaErrorInvalidValue;
+    }
+  }
+}
+
 // ---- moments -------------------------------------------------------------------------------------
 template <typename T, bool GRAIN, bool VEC, int NT>
 static cudaError_t launch_moments_k(const T* src, const PointParams& P, int row0, int rows, double* partials, float* fplanes, const LaunchCtx& ctx) {
@@ -219,6 +241,7 @@ cudaError_t launch_u8_out(const void* in, uint8_t* out, int64_t npix, const Laun
   template cudaError_t launch_lut_rgba<T>(const void*, void*, int64_t, const LutParams&, const LaunchCtx&);               \
   template cudaError_t launch_tile<T>(const CUtensorMap*, const void*, void*, TileParams&, int, bool, const LaunchCtx&);  \
   template cudaError_t launch_tile_rgba<T>(const CUtensorMap*, const void*, void*, TileParams&, const LaunchCtx&);        \
+  template cudaError_t launch_tile_rgba_lut<T>(const CUtensorMap*, const void*, void*, TileParams&, const LaunchCtx&);    \
   template cudaError_t launch_moments<T>(const void*, const PointParams&, bool, int, int, double*, double*, const LaunchCtx&, float*, bool); \
   template cudaError_t launch_adjust<T>(const void*, void*, const AdjustParams&, int, float*, float*, const LaunchCtx&);              \
   template cudaError_t launch_resize<T>(const void*, void*, const ResizeParams&, const LaunchCtx&);                       \

@@ -4,8 +4,9 @@
 //   k_point : streaming per-pixel chain  [grain][colour match][3D LUT]          (no neighbourhood)
 //   k_tile  : TMA-staged halo tiles      [grain][colour match][3D LUT] -> 3x3 stencil -> [post grain]
 // plus the LAB moment reduction and the uint8 wire-format codecs.
-// Data layout: frames [B][H][W][3] channel-fastest; a frame row is RW = 3*W contiguous elements.  The plain stencil of k_tile also
-// reads RGBA frames [B][H][W][4] interleaved as they are stored (CH = 4: RW = 4*W, neighbours e±4); every other kernel is RGB.
+// Data layout: frames [B][H][W][3] channel-fastest; a frame row is RW = 3*W contiguous elements.  k_tile also reads RGBA frames
+// [B][H][W][4] interleaved as they are stored (CH = 4: RW = 4*W, neighbours e±4), for the stencil with or without the 3D LUT in
+// front of it; k_lut_rgba is the LUT alone on RGBA; every other kernel is RGB.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -339,10 +340,13 @@ struct TileParams {
 // Everything else uses 256-thread CTAs, a 3-stage ring and 2 CTAs per SM.
 // WORK = 16-bit frames with pre-stages: their fp32 results live in a separate work tile, and a thread then produces
 // 4 elements per row (16-byte shared loads at a 16-byte lane stride are bank-conflict free; 32-byte strides are not).
-// CH = channels per pixel: the stencil's neighbours are e±CH.  CH = 4 (RGBA) exists for the plain stencil on float frames only:
-// the pre-stages and the post grain work on RGB pixel pairs, and byte frames are the 3-channel BGR wire format.
+// CH = channels per pixel: the stencil's neighbours are e±CH and a pre-stage pixel pair is 2*CH elements.  CH = 4 (RGBA) exists on
+// float frames for the plain stencil and for the 3D LUT in front of it (the stages the reference defines on RGBA: the LUT grades RGB
+// and carries alpha, the NumPy-path sharpeners filter every channel); grain, colour match and post grain are RGB stages, and byte
+// frames are the 3-channel BGR wire format.
 template <typename T, int MASK, int CH = 3> struct TileCfg {
-  static_assert(CH == 3 || (CH == 4 && MASK == 0 && sizeof(T) != 1), "4-channel tiles: plain stencil on fp32 / fp16 / bf16 frames");
+  static_assert(CH == 3 || (CH == 4 && (MASK == 0 || MASK == ST_LUT) && sizeof(T) != 1),
+                "4-channel tiles: plain stencil or LUT + stencil on fp32 / fp16 / bf16 frames");
   static constexpr int NCH = CH;
   static constexpr bool HEAVY = (MASK & ST_LUT) != 0;
   static constexpr bool WORK = (sizeof(T) == 1) || (((MASK & ST_PRE) != 0) && (sizeof(T) != 4));   // uint8 frames always convert into the work tile
@@ -369,7 +373,7 @@ template <typename T, int MASK, int CH = 3> struct TileCfg {
   static constexpr int COLS = TXE / VEC;              // threads across
   static constexpr int RG = (THREADS / COLS) >= 8 ? 8 : 4;   // row groups: COLS*RG active threads
   static constexpr int RPT = TY / RG;                 // rows per thread
-  static constexpr int PPR = TXE / 3 + 2;             // halo-tile pixels per row
+  static constexpr int PPR = TXE / CH + 2;            // halo-tile pixels per row
   static constexpr int PAIRS = PPR / 2 + 1;           // generator pixel pairs covering them (tile x origin is even)
   // pipeline stages; in-place (fp32) LUT tiles need the staged tile until the stencil is done, so they keep a second stage
   static constexpr int NS = HEAVY ? (WORK ? 1 : 2) : ((GPLANE || SLIM) ? 2 : 3);
@@ -377,6 +381,7 @@ template <typename T, int MASK, int CH = 3> struct TileCfg {
   static_assert(PADL + TXE + CH <= BX, "box too narrow: the right halo pixel must lie inside the box");
   static_assert(PADL >= CH, "the left halo pixel must lie inside the box's 16-byte left pad");
   static_assert(TXE % CH == 0 && TXE % VEC == 0, "tiles start on a pixel and on a thread's output run");
+  static_assert(TXE % (2 * CH) == 0, "tiles start on a pixel pair");
   static_assert(TY % RG == 0 && COLS * RG <= THREADS, "thread mapping");
 };
 
@@ -552,7 +557,7 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
           o[4 * q] = clamp01(fmaf(Q.pI, gv.x, o[4 * q])); o[4 * q + 1] = clamp01(fmaf(Q.pI, gv.y, o[4 * q + 1]));
           o[4 * q + 2] = clamp01(fmaf(Q.pI, gv.z, o[4 * q + 2])); o[4 * q + 3] = clamp01(fmaf(Q.pI, gv.w, o[4 * q + 3]));
         }
-      } else if ((MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<VEC, Io<T>::BGR>(Q, pgf, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
+      } else if (CH == 3 && (MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<VEC, Io<T>::BGR>(Q, pgf, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
       store_elems<T, VEC>(out, Q, frame, y, ge0, o);
     }
   } else {
@@ -578,7 +583,7 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
           o[4 * q] = clamp01(fmaf(Q.pI, gv.x, o[4 * q])); o[4 * q + 1] = clamp01(fmaf(Q.pI, gv.y, o[4 * q + 1]));
           o[4 * q + 2] = clamp01(fmaf(Q.pI, gv.z, o[4 * q + 2])); o[4 * q + 3] = clamp01(fmaf(Q.pI, gv.w, o[4 * q + 3]));
         }
-      } else if ((MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<VEC, Io<T>::BGR>(Q, pgf, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
+      } else if (CH == 3 && (MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<VEC, Io<T>::BGR>(Q, pgf, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
       store_elems<T, VEC>(out, Q, frame, y, ge0, o);
 #pragma unroll
       for (int i = 0; i < WN; ++i) { w[0][i] = w[1][i]; w[1][i] = w[2][i]; }
@@ -615,8 +620,72 @@ __device__ __forceinline__ void pair_store6(float* p, bool word0, const float* e
   q[2] = make_float2(e[4], e[5]);
 }
 
-// CH = 4: RGBA frames, plain stencil only (MASK 0); EXACT then selects the stencil arithmetic (exact on fp32 frames, fast on 16-bit
-// ones: the rule of the 3-channel stencil) and Q.op is one of the NumPy-path ops 1, 2, 4 (launch_tile_rgba).
+// eight consecutive staged elements (two RGBA pixels, 16-byte aligned for fp32, 8-byte for 16-bit) as two 4-element words
+template <typename T>
+__device__ __forceinline__ void pair_load8(const T* p, bool word0, float* e) {
+  if (sizeof(T) == 4) {
+    const float4* q = reinterpret_cast<const float4*>(p);
+    if (word0) { const float4 v = q[0]; e[0] = v.x; e[1] = v.y; e[2] = v.z; e[3] = v.w; }
+    const float4 v1 = q[1];
+    e[4] = v1.x; e[5] = v1.y; e[6] = v1.z; e[7] = v1.w;
+  } else {
+    const uint2* q = reinterpret_cast<const uint2*>(p);
+    union { uint2 u[2]; T h[8]; } w;
+    w.u[0] = word0 ? q[0] : make_uint2(0u, 0u); w.u[1] = q[1];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) e[i] = Elem<T>::ld(w.h[i]);
+  }
+}
+__device__ __forceinline__ void pair_store8(float* p, bool word0, const float* e) {
+  float4* q = reinterpret_cast<float4*>(p);
+  if (word0) q[0] = make_float4(e[0], e[1], e[2], e[3]);
+  q[1] = make_float4(e[4], e[5], e[6], e[7]);
+}
+
+// LUT pre-stage of an RGBA halo tile (CH = 4).  One task = one pixel pair = 8 staged elements, pixel a then pixel b (pixel a lies
+// left of the box when kx == 0).  The RGB of both pixels go through lut_pair as in the 3-channel pre-stage; alpha is carried the way
+// k_lut_rgba carries it: copied at blend 1, otherwise a*(1-blend) + a*blend with one rounding per operation.  fp32 tiles are
+// modified in place; 16-bit tiles are converted into the fp32 work tile, alpha included, with zeros for pixels outside the image.
+template <typename T, typename C, bool EXACT>
+__device__ __forceinline__ void lut_prestage_rgba(const TileParams& Q, T* raw, float* work, int y0, int x0e) {
+  constexpr int CH = 4, BX = C::BX, PADL = C::PADL, PAIRS = C::PAIRS, TASKS = C::ROWS * PAIRS;
+  const LutParams& L = Q.P.lut;
+  const int tid = threadIdx.x;
+  const int pair0 = x0e / (2 * CH) - 1;                    // pair holding the left halo pixel (x0e is a multiple of TXE, TXE of 8)
+  // whole warps walk the tasks (the LUT gather shuffles between lanes): a lane past the last task computes on zeros and stores nothing
+  for (int i0 = tid & ~31; i0 < TASKS; i0 += C::THREADS) {
+    const int i = i0 + (tid & 31);
+    const bool task = i < TASKS;
+    const int r = i / PAIRS, kx = i - r * PAIRS;
+    const int y = y0 - 1 + r, pxa = (pair0 + kx) * 2;
+    const int so = r * BX + PADL - 2 * CH + 2 * CH * kx;   // smem element of pixel a
+    const bool rowin = task && (y >= 0 && y < Q.H);
+    const bool in_a = (kx > 0) && rowin && pxa >= 0 && pxa < Q.W;
+    const bool in_b = (kx < PAIRS - 1) && rowin && pxa + 1 >= 0 && pxa + 1 < Q.W;
+    float e[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (in_a | in_b) pair_load8<T>(raw + so, kx > 0, e);
+    float p[6] = {e[0], e[1], e[2], e[4], e[5], e[6]};
+    lut_pair<EXACT, true>(Q.P, p);                         // every lane: lanes without pixels in the image serve their partner
+    const bool mix = L.blend < 1.0f;
+    if (in_a) {
+      e[0] = p[0]; e[1] = p[1]; e[2] = p[2];
+      if (mix) e[3] = lut_blend<EXACT>(e[3], e[3], L.blend, L.one_minus_blend);
+    } else if (C::WORK) { e[0] = 0.f; e[1] = 0.f; e[2] = 0.f; e[3] = 0.f; }
+    if (in_b) {
+      e[4] = p[3]; e[5] = p[4]; e[6] = p[5];
+      if (mix) e[7] = lut_blend<EXACT>(e[7], e[7], L.blend, L.one_minus_blend);
+    } else if (C::WORK) { e[4] = 0.f; e[5] = 0.f; e[6] = 0.f; e[7] = 0.f; }
+    if constexpr (C::WORK) {
+      if (task) pair_store8(work + so, kx > 0, e);
+    } else {
+      if (in_a | in_b) pair_store8(reinterpret_cast<float*>(raw) + so, kx > 0, e);   // in place; untouched pixels keep their staged value
+    }
+  }
+}
+
+// CH = 4: RGBA frames, the plain stencil (MASK 0) or the LUT + stencil (MASK ST_LUT), Q.op one of the NumPy-path ops 1, 2, 4.  With
+// MASK 0, EXACT selects the stencil arithmetic (exact on fp32 frames, fast on 16-bit ones: the rule of the 3-channel stencil,
+// launch_tile_rgba); with the LUT, EXACT is the LUT's arithmetic and the stencil follows the same per-dtype rule (launch_tile_rgba_lut).
 template <typename T, int MASK, bool EXACT, int CH = 3>
 __global__ void __launch_bounds__((TileCfg<T, MASK, CH>::LB_THREADS), (TileCfg<T, MASK, CH>::MINB))
 k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __restrict__ out, TileParams Q) {
@@ -705,7 +774,14 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
 
     // ---- per-pixel pre-stages over the halo tile (grain / colour match / LUT), result in fp32 ----
     // one task = one generator pixel pair (2 horizontally adjacent pixels): one Philox call, two independent LUT gathers in flight
-    if ((MASK & ST_PRE) != 0 || WORK || GPLANE) {
+    if constexpr (CH == 4 && (MASK & ST_LUT) != 0) {
+      lut_prestage_rgba<T, C, EXACT>(Q, raw, work, y0, x0e);
+      __syncthreads();
+      if (EARLY && tma && tid == 0 && k + NS < n_my) {
+        fence_proxy_async();          // the pre-stage's generic-proxy reads of this stage happen-before the async refill
+        issue(k + NS);
+      }
+    } else if ((MASK & ST_PRE) != 0 || WORK || GPLANE) {
       const PointParams& P = Q.P;
       constexpr bool GRAIN = (MASK & ST_GRAIN) != 0;
       constexpr bool BGR = Io<T>::BGR;
@@ -792,10 +868,11 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
     {
       const float* wt = WORK ? work : nullptr;
       if constexpr (CH != 3) {
+        constexpr bool XS = (MASK == 0) ? EXACT : (sizeof(T) == 4);
         switch (Q.op) {
-          case 1: stencil_rows<T, 1, MASK, EXACT, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 2: stencil_rows<T, 2, MASK, EXACT, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          default: stencil_rows<T, 4, MASK, EXACT, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 1: stencil_rows<T, 1, MASK, XS, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 2: stencil_rows<T, 2, MASK, XS, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          default: stencil_rows<T, 4, MASK, XS, CH>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
         }
       } else if (Q.exact_stencil) {   // uniform; one specialised row loop per epilogue and arithmetic variant
         switch (Q.op) {
@@ -1062,6 +1139,8 @@ template <typename T> cudaError_t launch_tile(const CUtensorMap* tmap, const voi
                                               bool exact, const LaunchCtx& ctx);
 template <typename T> cudaError_t launch_tile_rgba(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q,
                                                    const LaunchCtx& ctx);
+template <typename T> cudaError_t launch_tile_rgba_lut(const CUtensorMap* tmap, const void* in, void* out, TileParams& Q,
+                                                       const LaunchCtx& ctx);
 template <typename T> cudaError_t launch_moments(const void* in, const PointParams& P, bool grain, int row0, int rows,
                                                  double* sums, double* partials, const LaunchCtx& ctx, float* fplanes = nullptr,
                                                  bool small_blocks = false);

@@ -172,13 +172,21 @@ def _check_out(out, t):
 
 
 def chain_apply(images, desc, ext_noise=None, keepalive=(), out=None, fast_math=False):
-    """Run the fused chain described by a ChainDesc.  `keepalive` holds tensors the descriptor points to."""
-    t = _frames(images)
-    B, H, W, _ = t.shape
+    """Run the fused chain described by a ChainDesc.  `keepalive` holds tensors the descriptor points to.  images [B,H,W,3|4]: RGBA
+    frames take the LUT and the NumPy-path stencils only (vrgdg_chain_apply_ch), and no external noise."""
+    t = nv.require_cuda(images, "images")
+    if t.ndim != 4 or t.shape[-1] not in (3, 4):
+        raise ValueError("vrgdg_b200: images must be shaped [batch, height, width, 3 or 4], got %s" % (tuple(t.shape),))
+    B, H, W, C = t.shape
+    if C == 4 and ext_noise is not None:
+        raise ValueError("vrgdg_b200: ext_noise feeds the grain stage, which takes 3-channel frames; got 4 channels")
     out = torch.empty_like(t) if out is None else _check_out(out, t)
     lib = nv.load_library()
     with torch.cuda.device(t.device):
-        if ext_noise is not None:
+        if C == 4:
+            nv.check(lib.vrgdg_chain_apply_ch(nv.ptr(t), nv.ptr(out), B, H, W, 4, nv.DTYPE_CODE[t.dtype], ctypes.byref(desc),
+                                              nv.stream_ptr(t.device)))
+        elif ext_noise is not None:
             n = _noise(ext_noise, t)
             nv.check(lib.vrgdg_chain_apply_ext(nv.ptr(t), nv.ptr(out), B, H, W, nv.DTYPE_CODE[t.dtype], ctypes.byref(desc), nv.ptr(n),
                                                nv.CHAIN_FAST_MATH if fast_math else 0, nv.stream_ptr(t.device)))

@@ -185,6 +185,19 @@ typedef struct vrgdg_chain_desc {
 VRGDG_API int vrgdg_chain_apply(const void* in, void* out, int B, int H, int W, int dtype,
                       const vrgdg_chain_desc* desc, void* stream);
 
+/* vrgdg_chain_apply on frames [B,H,W,channels].  channels 3 is vrgdg_chain_apply.  channels 4 (RGBA IMAGE tensors) runs the
+ * stages the reference defines on 4 channels, in one pass when both are enabled: the 3D LUT grades RGB and carries alpha
+ * (VRGDG_IV_Adjustments.py:341-343: copied at lut_blend 1, otherwise a*(1-blend) + a*blend like every channel), then the stencil
+ * filters every channel, alpha included, as vrgdg_stencil3x3_ch does.  The result is the reference's VRGDG_LUTS -> sharpener
+ * composition on fp32 tensors, bit for bit on fp32 frames; on 16-bit frames the LUT result stays fp32 up to the stencil, and the
+ * RGB channels equal the 3-channel chain's on the same RGB bit for bit.  Nothing enabled copies, the LUT alone is vrgdg_lut3d_apply
+ * with 4 channels, the stencil alone vrgdg_stencil3x3_ch.
+ * Checked before any CUDA call: other channel counts are VRGDG_E_INVALID; uint8 frames, grain, colour match or post grain enabled,
+ * and the torch-path ops VRGDG_STENCIL_LAPLACIAN_GPU / _SOBEL_GPU are VRGDG_E_UNSUPPORTED (the reference raises on 4 channels
+ * there); in == out with a stencil is VRGDG_E_INVALID; an empty batch is a successful no-op. */
+VRGDG_API int vrgdg_chain_apply_ch(const void* in, void* out, int B, int H, int W, int channels, int dtype,
+                         const vrgdg_chain_desc* desc, void* stream);
+
 /* vrgdg_chain_apply with the first grain stage reading N(0,1) from ext_noise ([B,H,W,3], frame dtype) instead
  * of the in-kernel generator: lets the fused chain be compared with the reference composition on the same
  * noise tensor (nodes.py:51 draws it from torch's generator, which no CUDA kernel can reproduce). */
