@@ -21,6 +21,9 @@ DTYPE_CODE = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16, torc
 STENCIL_NONE, STENCIL_BOX_UNSHARP, STENCIL_LAPLACIAN_CPU, STENCIL_LAPLACIAN_GPU, STENCIL_SOBEL_CPU, STENCIL_SOBEL_GPU = range(6)
 BORDER_REPLICATE, BORDER_ZERO = 0, 1
 SEED_PER_CLIP, SEED_PER_FRAME = 0, 1
+# torch's CUDA randn stream of a fresh seeded generator (include/vrgdg_b200.h): one [H,W,3] draw per frame seeded
+# (seed + frame0 + i) & 0x7FFFFFFF, or one [B,H,W,3] draw per call seeded `seed`
+SEED_TORCH_PER_FRAME, SEED_TORCH_PER_CALL = 2, 3
 CHAIN_FAST_MATH = 1
 CHAIN_CM_RECOMPUTE = 2
 CHAIN_CM_SERIAL = 4

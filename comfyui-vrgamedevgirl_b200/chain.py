@@ -18,7 +18,8 @@ from ._runtime import compute_device, cuda_device, stream_frames, stream_frames_
 class PostChain:
     def __init__(self, grain=None, colormatch=None, lut=None, stencil=None, post_grain=None, device=None, devices=None):
         """
-        grain / post_grain: dict(intensity, saturation_mix, seed, seed_mode=SEED_PER_CLIP)
+        grain / post_grain: dict(intensity, saturation_mix, seed, seed_mode=SEED_PER_CLIP); post_grain also takes
+                            seed_mode=SEED_TORCH_PER_FRAME (torch's CUDA randn stream of the enhancer's per-frame seeded generators)
         colormatch:         dict(reference_image=[1,H,W,3] tensor  |  ref_sums=[1,7] float64, strength)
         lut:                dict(lut_data={"lut","domain_min","domain_max"}, strength 0..10)
         stencil:            dict(op=STENCIL_*, strength, border=BORDER_REPLICATE)

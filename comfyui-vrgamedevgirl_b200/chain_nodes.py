@@ -105,7 +105,12 @@ class VRGDG_B200_EnhanceFrames:
                 "seed": ("INT", {"default": 42, "min": 0, "max": 0x7FFFFFFF}),
                 "frame_start": ("INT", {"default": 0, "min": 0, "max": 0x7FFFFFFF}),
                 "use_gpu": ("BOOLEAN", {"default": True, "tooltip": "the enhancer's setting of the same name: True = zero-padded box blur (avg_pool2d), False = edge-replicated"}),
-            }
+            },
+            "optional": {
+                "noise_stream": (["vrgdg", "torch_cuda"], {"default": "vrgdg", "tooltip": "vrgdg = this package's grain generator; torch_cuda = "
+                                 "torch's CUDA randn stream of the enhancer's per-frame seeded generators: the same grain as the reference "
+                                 "rendering on the same GPU model"}),
+            },
         }
 
     RETURN_TYPES = ("IMAGE",)
@@ -113,12 +118,14 @@ class VRGDG_B200_EnhanceFrames:
     CATEGORY = "VRGDG/Video"
     DESCRIPTION = "Unsharp + per-frame seeded film grain (the standalone enhancer's effect chain) on an IMAGE batch."
 
-    def enhance(self, images, sharpen_strength, grain_intensity, saturation_mix, seed, frame_start, use_gpu):
+    def enhance(self, images, sharpen_strength, grain_intensity, saturation_mix, seed, frame_start, use_gpu, noise_stream="vrgdg"):
+        from .video_tools import _seed_mode
+        mode = _seed_mode(noise_stream, nv.SEED_PER_FRAME, nv.SEED_TORCH_PER_FRAME)
         images = _as_frames(images)
         dev = compute_device(images)
         stencil = dict(op=nv.STENCIL_BOX_UNSHARP, strength=float(sharpen_strength), border=nv.BORDER_ZERO if use_gpu else nv.BORDER_REPLICATE) \
             if float(sharpen_strength) > 0 else None
-        post = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), seed=int(seed), seed_mode=nv.SEED_PER_FRAME) \
+        post = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), seed=int(seed), seed_mode=mode) \
             if float(grain_intensity) > 0 else None
         if stencil is None and post is None:
             return (images,)
@@ -127,7 +134,7 @@ class VRGDG_B200_EnhanceFrames:
             from . import ops
             s = post["saturation_mix"]
             make_fn = lambda d: lambda f, i: ops.grain(f, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start) + i,
-                                                       seed_mode=nv.SEED_PER_FRAME)
+                                                       seed_mode=mode)
         else:
             make_fn = PostChain(stencil=stencil, post_grain=post, device=None if devs else dev, devices=devs).make_fn(int(frame_start))
         return (run_frames(images, make_fn, 8, result_device(images), devs[0] if devs else dev, devs),)

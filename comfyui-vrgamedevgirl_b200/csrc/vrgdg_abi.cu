@@ -44,19 +44,55 @@ int get_ctx(void* stream, LaunchCtx& ctx) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return fail_cuda(e, "cudaGetDevice");
-  static thread_local int cached_dev = -1, cached_sms = 0, cached_major = 0, cached_minor = 0;
+  static thread_local int cached_dev = -1, cached_sms = 0, cached_major = 0, cached_minor = 0, cached_tpsm = 0;
   if (cached_dev != dev) {
-    int sms = 0, major = 0, minor = 0;
+    int sms = 0, major = 0, minor = 0, tpsm = 0;
     if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
     if ((e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
     if ((e = cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
-    cached_dev = dev; cached_sms = sms; cached_major = major; cached_minor = minor;
+    if ((e = cudaDeviceGetAttribute(&tpsm, cudaDevAttrMaxThreadsPerMultiProcessor, dev)) != cudaSuccess) return fail_cuda(e, "cudaDeviceGetAttribute");
+    cached_dev = dev; cached_sms = sms; cached_major = major; cached_minor = minor; cached_tpsm = tpsm;
   }
   if (cached_major != 9 || cached_minor != 0)   // sm_90a code runs on compute capability 9.0 only
     return fail(VRGDG_E_UNSUPPORTED, "libvrgdg_b200 holds sm_90a code only; device %d has compute capability %d.%d", dev, cached_major,
                 cached_minor);
   ctx.stream = reinterpret_cast<cudaStream_t>(stream);
   ctx.sms = cached_sms;
+  ctx.threads_per_sm = cached_tpsm;
+  return VRGDG_OK;
+}
+
+// ---- torch-stream grain (VRGDG_SEED_TORCH_*) ---------------------------------------------------------
+bool seed_mode_ok(int m) { return m == VRGDG_SEED_PER_CLIP || m == VRGDG_SEED_PER_FRAME || m == VRGDG_SEED_TORCH_PER_FRAME || m == VRGDG_SEED_TORCH_PER_CALL; }
+bool torch_mode(int m) { return m == VRGDG_SEED_TORCH_PER_FRAME || m == VRGDG_SEED_TORCH_PER_CALL; }
+
+// elements of one draw: [H,W,3] per frame, or [B,H,W,3] per call
+int64_t torch_draw_numel(int B, int H, int W, int seed_mode) {
+  return (int64_t)(seed_mode == VRGDG_SEED_TORCH_PER_CALL ? B : 1) * H * W * 3;
+}
+
+// ATen splits a draw whose byte extent needs 64-bit indexing (TensorIterator::can_use_32bit_indexing) into sub-draws with Philox
+// offsets of their own; that stream is not reproduced.  draw_es: element size of the reference's noise tensor.
+int check_torch_draw(int64_t numel, size_t draw_es, const char* who) {
+  if (numel > 0 && 1 + (numel - 1) * (int64_t)draw_es > (int64_t)INT32_MAX)
+    return fail(VRGDG_E_UNSUPPORTED, "%s: a torch-stream draw of %lld elements of %d bytes exceeds 32-bit indexing (torch splits it into "
+                "sub-draws, which is not reproduced); split the batch", who, (long long)numel, (int)draw_es);
+  return VRGDG_OK;
+}
+
+// the reference draws the noise in the frame dtype; uint8 frames become fp32 tensors first
+size_t torch_draw_es(int dtype) { return dtype == VRGDG_U8BGR ? 4 : (dtype == VRGDG_F32 ? 4 : 2); }
+
+// Torch-stream refusals of the chain entry points, checked before any CUDA call: the first grain stage draws from the global generator
+// in the reference (FastFilmGrain), per-call draws have no post-grain counterpart, and post-grain draws must fit 32-bit indexing.
+int check_chain_torch(const vrgdg_chain_desc* d, int H, int W, int dtype, const char* who) {
+  if (d->grain_enabled && torch_mode(d->grain_seed_mode))
+    return fail(VRGDG_E_UNSUPPORTED, "%s: the first grain stage takes VRGDG_SEED_PER_CLIP / _PER_FRAME; torch-stream modes are for "
+                "vrgdg_grain and the post-grain stage", who);
+  if (d->post_grain_enabled && d->post_seed_mode == VRGDG_SEED_TORCH_PER_CALL)
+    return fail(VRGDG_E_UNSUPPORTED, "%s: post grain takes VRGDG_SEED_TORCH_PER_FRAME, not _PER_CALL", who);
+  if (d->post_grain_enabled && d->post_seed_mode == VRGDG_SEED_TORCH_PER_FRAME)
+    return check_torch_draw((int64_t)H * W * 3, torch_draw_es(dtype), who);
   return VRGDG_OK;
 }
 
@@ -256,8 +292,10 @@ int vrgdg_grain(const void* in, void* out, int B, int H, int W, int dtype, float
                 uint64_t seed, int64_t frame0, int seed_mode, const void* ext_noise, void* stream) {
   int rc = check_frames(in, out, B, H, W, dtype, "vrgdg_grain");
   if (rc) return rc;
-  if (seed_mode != VRGDG_SEED_PER_CLIP && seed_mode != VRGDG_SEED_PER_FRAME) return fail(VRGDG_E_INVALID, "vrgdg_grain: bad seed_mode %d", seed_mode);
+  if (!seed_mode_ok(seed_mode)) return fail(VRGDG_E_INVALID, "vrgdg_grain: bad seed_mode %d", seed_mode);
   if ((int64_t)B * H * W == 0) return VRGDG_OK;
+  const bool torch = torch_mode(seed_mode) && ext_noise == nullptr;
+  if (torch && (rc = check_torch_draw(torch_draw_numel(B, H, W, seed_mode), torch_draw_es(dtype), "vrgdg_grain"))) return rc;
   LaunchCtx ctx;
   if ((rc = get_ctx(stream, ctx))) return rc;
   PointParams P;
@@ -265,7 +303,8 @@ int vrgdg_grain(const void* in, void* out, int B, int H, int W, int dtype, float
   P.gI = intensity; P.gs = sat; P.goms = one_minus_sat;
   P.seed = seed; P.frame0 = frame0; P.seed_mode = seed_mode; P.ext_noise = ext_noise;
   grain_make_key(seed, seed_mode, P.gkey);
-  const bool exact = ext_noise != nullptr;
+  if (torch) P.tT = torch_randn_threads((uint64_t)torch_draw_numel(B, H, W, seed_mode), ctx.sms, ctx.threads_per_sm);
+  const bool exact = ext_noise != nullptr || torch;   // the torch stream always takes the reference's op order
 #define PT(T) launch_point<T>(in, out, P, ST_GRAIN, exact, ctx)
   cudaError_t e = DISPATCH_DTYPE(dtype, PT);
 #undef PT
@@ -277,15 +316,17 @@ int vrgdg_grain_noise(float* out, int B, int H, int W, uint64_t seed, int64_t fr
   if (B < 0 || H < 0 || W < 0) return fail(VRGDG_E_INVALID, "vrgdg_grain_noise: negative shape");
   if ((int64_t)B * H * W == 0) return VRGDG_OK;
   if (!out) return fail(VRGDG_E_INVALID, "vrgdg_grain_noise: null output");
+  if (!seed_mode_ok(seed_mode)) return fail(VRGDG_E_INVALID, "vrgdg_grain_noise: bad seed_mode %d", seed_mode);
+  int rc;
+  if (torch_mode(seed_mode) && (rc = check_torch_draw(torch_draw_numel(B, H, W, seed_mode), 4, "vrgdg_grain_noise"))) return rc;
   LaunchCtx ctx;
-  int rc = get_ctx(stream, ctx);
-  if (rc) return rc;
+  if ((rc = get_ctx(stream, ctx))) return rc;
   int64_t total = (int64_t)B * H * W;
   int grid = (int)(((total + 255) / 256) < (int64_t)ctx.sms * 16 ? ((total + 255) / 256) : (int64_t)ctx.sms * 16);
-  if (seed_mode != VRGDG_SEED_PER_CLIP && seed_mode != VRGDG_SEED_PER_FRAME) return fail(VRGDG_E_INVALID, "vrgdg_grain_noise: bad seed_mode %d", seed_mode);
   GrainKey K;
   grain_make_key(seed, seed_mode, K);
-  k_grain_noise<<<grid, 256, 0, ctx.stream>>>(out, B, W, (int64_t)H * W, seed, frame0, seed_mode, K);
+  const uint32_t nT = torch_mode(seed_mode) ? torch_randn_threads((uint64_t)torch_draw_numel(B, H, W, seed_mode), ctx.sms, ctx.threads_per_sm) : 0u;
+  k_grain_noise<<<grid, 256, 0, ctx.stream>>>(out, B, W, (int64_t)H * W, seed, frame0, seed_mode, K, nT);
   count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail_cuda(e, "vrgdg_grain_noise");
@@ -427,7 +468,8 @@ static int chain_apply_core(const void* in, void* out, int B, int H, int W, int 
   if (rc) return rc;
   if (d->stencil_op < VRGDG_STENCIL_NONE || d->stencil_op > VRGDG_STENCIL_SOBEL_GPU) return fail(VRGDG_E_INVALID, "chain: bad stencil op %d", d->stencil_op);
   if (d->stencil_border != VRGDG_BORDER_REPLICATE && d->stencil_border != VRGDG_BORDER_ZERO) return fail(VRGDG_E_INVALID, "chain: bad border %d", d->stencil_border);
-  if (d->post_grain_enabled && d->post_seed_mode != VRGDG_SEED_PER_CLIP && d->post_seed_mode != VRGDG_SEED_PER_FRAME) return fail(VRGDG_E_INVALID, "chain: bad post seed_mode");
+  if (d->post_grain_enabled && !seed_mode_ok(d->post_seed_mode)) return fail(VRGDG_E_INVALID, "chain: bad post seed_mode");
+  if ((rc = check_chain_torch(d, H, W, dtype, "vrgdg_chain_apply"))) return rc;
   if ((int64_t)B * H * W == 0) return VRGDG_OK;
   LaunchCtx ctx;
   if ((rc = get_ctx(stream, ctx))) return rc;
@@ -466,6 +508,12 @@ static int chain_apply_core(const void* in, void* out, int B, int H, int W, int 
   Q.pI = dd.post_intensity; Q.ps = dd.post_sat; Q.poms = dd.post_one_minus_sat;
   Q.pseed = dd.post_seed; Q.pframe0 = dd.post_frame0; Q.pseed_mode = dd.post_seed_mode;
   grain_make_key(Q.pseed, Q.pseed_mode, Q.pkey);
+  if (Q.post_enabled && dd.post_seed_mode == VRGDG_SEED_TORCH_PER_FRAME) {
+    // torch-stream post grain exists in the exact instantiations only (the reference's op order, one rounding per op)
+    Q.ptT = torch_randn_threads((uint64_t)H * W * 3, ctx.sms, ctx.threads_per_sm);
+    exact = true;
+    Q.exact_stencil = (dtype == VRGDG_F32 || dtype == VRGDG_U8BGR) ? 1 : 0;
+  }
   if (Q.post_enabled && mask == 0) mask = ST_POST;    // pure stencil + post grain: one Philox call per pixel pair via the grain plane
   return run_tile(in, out, B, H, W, 3, dtype, Q, mask, exact, ctx);
 }
@@ -539,6 +587,7 @@ int vrgdg_chain_apply_ch(const void* in, void* out, int B, int H, int W, int cha
 static int chain_moments_impl(const void* in, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc, const void* ext_noise,
                               double* sums, void* scratch, int64_t scratch_bytes, void* stream, const char* who) {
   if (!desc) return fail(VRGDG_E_INVALID, "%s: null descriptor", who);
+  if (desc->grain_enabled && torch_mode(desc->grain_seed_mode)) return check_chain_torch(desc, H, W, dtype, who);
   if (B < 0 || H <= 0 || W <= 0) return fail(VRGDG_E_INVALID, "%s: bad shape", who);
   PointParams P;
   zero_point(P, B, H, W);
@@ -629,6 +678,7 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
   int rc = check_frames(in, out, B, H, W, dtype, "vrgdg_chain_cm_apply");
   if (rc) return rc;
   if (n_ref != 1 && n_ref != B) return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: reference batch %d is neither 1 nor %d", n_ref, B);
+  if ((rc = check_chain_torch(desc, H, W, dtype, "vrgdg_chain_cm_apply"))) return rc;
   if (desc->grain_enabled && desc->grain_seed_mode != VRGDG_SEED_PER_CLIP && desc->grain_seed_mode != VRGDG_SEED_PER_FRAME)
     return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: bad grain seed_mode %d", desc->grain_seed_mode);
   if ((int64_t)B * H * W == 0) return VRGDG_OK;

@@ -65,6 +65,13 @@ template <> struct Io<uint8_t> {
 template <typename T> __device__ __forceinline__ float noise_ld(T v) { return Elem<T>::ld(v); }
 template <> __device__ __forceinline__ float noise_ld<float>(float v) { return v; }
 
+// element li of a torch-stream draw as the reference's noise tensor holds it: cast to the frame dtype (round to nearest) for 16-bit
+// frames, fp32 for fp32 and uint8 frames (the reference's byte path works on fp32 tensors)
+template <typename T> __device__ __forceinline__ float torch_noise(uint64_t seed, uint32_t li, uint32_t nT) {
+  const float z = torch_randn(seed, li, nT);
+  return sizeof(T) == 2 ? Elem<T>::ld(Elem<T>::st(z)) : z;
+}
+
 // ---- parameters of the per-pixel stages ------------------------------------------------------------
 struct PointParams {
   int B, H, W;
@@ -75,6 +82,7 @@ struct PointParams {
   int64_t frame0;
   int seed_mode;
   GrainKey gkey;               // Philox round keys, evaluated on the host
+  uint32_t tT;                 // torch-stream modes: threads T of each draw (torch_randn_threads)
   const void* ext_noise;       // [B,H,W,3] of the frame dtype, or null
   // colour match
   const float* cm_params;      // [B][12]
@@ -148,6 +156,7 @@ k_point(const T* __restrict__ in, T* __restrict__ out, PointParams P,
   constexpr int NE = PX * 3;
   constexpr bool GRAIN = (MASK & ST_GRAIN) != 0;
   const bool has_ext = GRAIN && (P.ext_noise != nullptr);
+  const bool tstream = EXACT && GRAIN && torch_stream(P.seed_mode);   // torch's randn stream: exact blend only (host-enforced)
   for (int64_t vb = blockIdx.x; vb < total_vblocks; vb += gridDim.x) {
     const int frame = (int)(vb / blocks_per_frame);
     const int bif = (int)(vb - (int64_t)frame * blocks_per_frame);
@@ -187,6 +196,11 @@ k_point(const T* __restrict__ in, T* __restrict__ out, PointParams P,
 #pragma unroll
         for (int i = 0; i < NE; ++i) nz[i] = noise_ld<noise_t>(ns[i]);
       }
+    } else if (tstream) {   // the PX pixels lie in one frame: consecutive elements of its draw, RGB order
+      const uint64_t dseed = torch_draw_seed(P.seed, P.frame0, frame, P.seed_mode);
+      const uint32_t li0 = torch_draw_base(frame, P.hw, P.seed_mode) + (uint32_t)pix0 * 3u;
+#pragma unroll
+      for (int i = 0; i < NE; ++i) nz[i] = torch_noise<T>(dseed, li0 + (uint32_t)i, P.tT);
     }
     if (VEC) {
       // x is a multiple of PX (even): PX/2 whole generator pairs
@@ -194,7 +208,7 @@ k_point(const T* __restrict__ in, T* __restrict__ out, PointParams P,
       for (int j = 0; j < PX; j += 2) {
         float z[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         if (GRAIN) {
-          if (has_ext) {
+          if (has_ext || tstream) {
 #pragma unroll
             for (int i = 0; i < 6; ++i) z[i] = nz[3 * j + i];
           } else {
@@ -206,7 +220,7 @@ k_point(const T* __restrict__ in, T* __restrict__ out, PointParams P,
     } else {
       float zr = 0.f, zg = 0.f, zb = 0.f;
       if (GRAIN) {
-        if (has_ext) { zr = nz[0]; zg = nz[1]; zb = nz[2]; }
+        if (has_ext || tstream) { zr = nz[0]; zg = nz[1]; zb = nz[2]; }
         else grain_pixel_normals(P.gkey, gf, x, y, zr, zg, zb);
       }
       process_pixel<MASK, EXACT>(P, cmf, zr, zg, zb, v[0], v[1], v[2]);
@@ -247,13 +261,19 @@ k_lut_rgba(const T* __restrict__ in, T* __restrict__ out, int64_t npix, LutParam
   }
 }
 
-// raw normals of the generator, [B,H,W,3] fp32
+// raw normals of the generator, [B,H,W,3] fp32; torch-stream modes: nT = threads T of each draw
 static __global__ void __launch_bounds__(256)
-k_grain_noise(float* __restrict__ out, int B, int W, int64_t hw, uint64_t seed, int64_t frame0, int seed_mode, GrainKey K) {
+k_grain_noise(float* __restrict__ out, int B, int W, int64_t hw, uint64_t seed, int64_t frame0, int seed_mode, GrainKey K, uint32_t nT) {
   const int64_t total = (int64_t)B * hw;
   for (int64_t p = (int64_t)blockIdx.x * 256 + threadIdx.x; p < total; p += (int64_t)gridDim.x * 256) {
     int frame = (int)(p / hw);
     uint32_t pif = (uint32_t)(p - (int64_t)frame * hw);
+    if (torch_stream(seed_mode)) {
+      const uint64_t dseed = torch_draw_seed(seed, frame0, frame, seed_mode);
+      const uint32_t li0 = torch_draw_base(frame, hw, seed_mode) + pif * 3u;
+      out[p * 3] = torch_randn(dseed, li0, nT); out[p * 3 + 1] = torch_randn(dseed, li0 + 1u, nT); out[p * 3 + 2] = torch_randn(dseed, li0 + 2u, nT);
+      continue;
+    }
     uint32_t y = pif / (uint32_t)W, x = pif - y * (uint32_t)W;
     GrainFrame gf = grain_frame(seed, frame0, frame, seed_mode);
     float zr, zg, zb;
@@ -328,6 +348,7 @@ struct TileParams {
   int64_t pframe0;
   int pseed_mode;
   GrainKey pkey;                // round keys of the post-grain generator
+  uint32_t ptT;                 // VRGDG_SEED_TORCH_PER_FRAME: threads T of each frame's draw
   int exact_stencil;            // 1: reference evaluation order, one rounding per op (bit-exact NumPy-path results for fp32)
   int use_tma;                  // 0: cooperative bounds-checked loads (any alignment)
   int vec_store;                // rows 16-byte aligned -> 16-byte stores
@@ -456,9 +477,22 @@ __device__ __forceinline__ void load_window(const E* rowp /* -> tile column PADL
   }
 }
 
-// grain after the stencil (EnhancerNodes.py:285-293) on VEC consecutive row elements starting at element ge0
-template <int VEC, bool BGR>
-__device__ __forceinline__ void post_grain_elems(const TileParams& Q, const GrainFrame& gf, int ge0, int y, float* o) {
+// grain after the stencil (EnhancerNodes.py:285-293) on VEC consecutive row elements starting at element ge0.
+// EX (exact instantiations) and VRGDG_SEED_TORCH_PER_FRAME: element by element from torch's stream of the frame's draw (seed pds),
+// the reference's op order with one rounding per op.
+template <typename T, int VEC, bool BGR, bool EX>
+__device__ __forceinline__ void post_grain_elems(const TileParams& Q, const GrainFrame& gf, uint64_t pds, int ge0, int y, float* o) {
+  if (EX && Q.pseed_mode == SEED_TORCH_PER_FRAME) {
+#pragma unroll
+    for (int e = 0; e < VEC; ++e) {
+      const int ge = ge0 + e, px = ge / 3, cm = ge - px * 3, c = BGR ? 2 - cm : cm;
+      const uint32_t li3 = (uint32_t)((y * Q.W + px) * 3);
+      const float zc = torch_noise<T>(pds, li3 + (uint32_t)c, Q.ptT);
+      const float zg = (c == 1) ? zc : torch_noise<T>(pds, li3 + 1u, Q.ptT);
+      o[e] = clamp01(addx(o[e], mulx(grain_mix_exact(zc, zg, c, Q.ps, Q.poms), Q.pI)));
+    }
+    return;
+  }
   const int pfirst = ge0 / 3, plast = (ge0 + VEC - 1) / 3;
   constexpr int NPR = (VEC + 1) / 3 + 1;                    // pixel pairs a run of VEC elements can touch
 #pragma unroll
@@ -511,7 +545,7 @@ __device__ __forceinline__ void store_elems(T* __restrict__ out, const TileParam
   }
 }
 
-template <typename T, int OP, int MASK, bool XS, int CH = 3>
+template <typename T, int OP, int MASK, bool XS, int CH = 3, bool EX = false>
 __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, const float* gplane, T* __restrict__ out,
                                              const TileParams& Q, int frame, int y0, int x0e) {
   using C = TileCfg<T, MASK, CH>;
@@ -528,6 +562,9 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
     else load_window<T, VEC, CH>(raw + srow * BX + PADL + f0, dst);
   };
   const GrainFrame pgf = grain_frame(Q.pseed, Q.pframe0, frame, Q.pseed_mode);
+  const uint64_t pds = torch_draw_seed(Q.pseed, Q.pframe0, frame, Q.pseed_mode);
+  const bool ptorch = EX && Q.pseed_mode == SEED_TORCH_PER_FRAME;   // plane holds the exact mix: separate multiply and add
+  auto post_add = [&](float o, float g) { return ptorch ? clamp01(addx(o, mulx(g, Q.pI))) : clamp01(fmaf(Q.pI, g, o)); };
   if (OP == 1 && !XS) {
     // 3x3 box is separable: keep the horizontal 3-sums of the two previous rows (nodes.py:194-206)
     float h0[VEC], h1[VEC], c1[VEC], wr[WN];
@@ -554,10 +591,10 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
 #pragma unroll
         for (int q = 0; q < VEC / 4; ++q) {
           const float4 gv = gp[q];
-          o[4 * q] = clamp01(fmaf(Q.pI, gv.x, o[4 * q])); o[4 * q + 1] = clamp01(fmaf(Q.pI, gv.y, o[4 * q + 1]));
-          o[4 * q + 2] = clamp01(fmaf(Q.pI, gv.z, o[4 * q + 2])); o[4 * q + 3] = clamp01(fmaf(Q.pI, gv.w, o[4 * q + 3]));
+          o[4 * q] = post_add(o[4 * q], gv.x); o[4 * q + 1] = post_add(o[4 * q + 1], gv.y);
+          o[4 * q + 2] = post_add(o[4 * q + 2], gv.z); o[4 * q + 3] = post_add(o[4 * q + 3], gv.w);
         }
-      } else if (CH == 3 && (MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<VEC, Io<T>::BGR>(Q, pgf, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
+      } else if (CH == 3 && (MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<T, VEC, Io<T>::BGR, EX>(Q, pgf, pds, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
       store_elems<T, VEC>(out, Q, frame, y, ge0, o);
     }
   } else {
@@ -580,10 +617,10 @@ __device__ __forceinline__ void stencil_rows(const T* raw, const float* work, co
 #pragma unroll
         for (int q = 0; q < VEC / 4; ++q) {
           const float4 gv = gp[q];
-          o[4 * q] = clamp01(fmaf(Q.pI, gv.x, o[4 * q])); o[4 * q + 1] = clamp01(fmaf(Q.pI, gv.y, o[4 * q + 1]));
-          o[4 * q + 2] = clamp01(fmaf(Q.pI, gv.z, o[4 * q + 2])); o[4 * q + 3] = clamp01(fmaf(Q.pI, gv.w, o[4 * q + 3]));
+          o[4 * q] = post_add(o[4 * q], gv.x); o[4 * q + 1] = post_add(o[4 * q + 1], gv.y);
+          o[4 * q + 2] = post_add(o[4 * q + 2], gv.z); o[4 * q + 3] = post_add(o[4 * q + 3], gv.w);
         }
-      } else if (CH == 3 && (MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<VEC, Io<T>::BGR>(Q, pgf, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
+      } else if (CH == 3 && (MASK & ST_PRE) != 0 && Q.post_enabled) post_grain_elems<T, VEC, Io<T>::BGR, EX>(Q, pgf, pds, ge0, y, o);   // MASK 0 + post grain runs as ST_POST
       store_elems<T, VEC>(out, Q, frame, y, ge0, o);
 #pragma unroll
       for (int i = 0; i < WN; ++i) { w[0][i] = w[1][i]; w[1][i] = w[2][i]; }
@@ -810,7 +847,17 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
         if (GPLANE) {
           // post-grain values of this pair (added after the stencil): I*(s*z' + (1-s)*z_g) per element, memory channel order
           float gz[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-          if (rowin && pair >= 0 && pxa < Q.W) {
+          if (EXACT && rowin && pair >= 0 && pxa < Q.W && Q.pseed_mode == SEED_TORCH_PER_FRAME) {
+            const uint64_t pds = torch_draw_seed(Q.pseed, Q.pframe0, frame, Q.pseed_mode);
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              if (pxa + j >= Q.W) break;
+              const uint32_t li3 = (uint32_t)((y * Q.W + pxa + j) * 3);
+              const float zr = torch_noise<T>(pds, li3, Q.ptT), zg = torch_noise<T>(pds, li3 + 1u, Q.ptT), zb = torch_noise<T>(pds, li3 + 2u, Q.ptT);
+              const float gr = grain_mix_exact(zr, zg, 0, Q.ps, Q.poms), gg = grain_mix_exact(zg, zg, 1, Q.ps, Q.poms), gb = grain_mix_exact(zb, zg, 2, Q.ps, Q.poms);
+              gz[3 * j] = BGR ? gb : gr; gz[3 * j + 1] = gg; gz[3 * j + 2] = BGR ? gr : gb;
+            }
+          } else if (rowin && pair >= 0 && pxa < Q.W) {
             float z[6];
             grain_pair_normals(grain_pair_bits(Q.pkey, pgf, (uint32_t)pair, (uint32_t)y), z);
             const float gy0 = Q.poms * z[1], gy1 = Q.poms * z[4];
@@ -876,21 +923,21 @@ k_tile(const __grid_constant__ CUtensorMap tmap, const T* __restrict__ in, T* __
         }
       } else if (Q.exact_stencil) {   // uniform; one specialised row loop per epilogue and arithmetic variant
         switch (Q.op) {
-          case 1: stencil_rows<T, 1, MASK, true>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 2: stencil_rows<T, 2, MASK, true>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 3: stencil_rows<T, 3, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 4: stencil_rows<T, 4, MASK, true>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 5: stencil_rows<T, 5, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          default: stencil_rows<T, 0, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 1: stencil_rows<T, 1, MASK, true, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 2: stencil_rows<T, 2, MASK, true, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 3: stencil_rows<T, 3, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 4: stencil_rows<T, 4, MASK, true, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 5: stencil_rows<T, 5, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          default: stencil_rows<T, 0, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
         }
       } else {
         switch (Q.op) {
-          case 1: stencil_rows<T, 1, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 2: stencil_rows<T, 2, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 3: stencil_rows<T, 3, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 4: stencil_rows<T, 4, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          case 5: stencil_rows<T, 5, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
-          default: stencil_rows<T, 0, MASK, false>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 1: stencil_rows<T, 1, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 2: stencil_rows<T, 2, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 3: stencil_rows<T, 3, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 4: stencil_rows<T, 4, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          case 5: stencil_rows<T, 5, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
+          default: stencil_rows<T, 0, MASK, false, 3, EXACT>(raw, wt, gplane, out, Q, frame, y0, x0e); break;
         }
       }
     }
@@ -1129,7 +1176,7 @@ k_rgb_to_u8bgr(const T* __restrict__ in, uint8_t* __restrict__ out, int64_t npix
 }
 
 // ---- host-side launchers implemented per dtype translation unit (vrgdg_inst.cuh) --------------------
-struct LaunchCtx { cudaStream_t stream; int sms; };
+struct LaunchCtx { cudaStream_t stream; int sms; int threads_per_sm; };   // threads_per_sm: torch-stream draws (torch_randn_threads)
 
 template <typename T> cudaError_t launch_point(const void* in, void* out, const PointParams& P, int mask, bool exact,
                                                const LaunchCtx& ctx);

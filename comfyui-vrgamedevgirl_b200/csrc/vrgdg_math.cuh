@@ -196,6 +196,102 @@ VRGDG_HD void grain_pixel_normals(const GrainKey& K, const GrainFrame& f, uint32
   grain_lane_normals(grain_pair_bits(K, f, x >> 1, y), (int)(x & 1u), zr, zg, zb);
 }
 
+// ---- torch's CUDA randn stream (VRGDG_SEED_TORCH_PER_FRAME / _PER_CALL) -----------------------------------
+// torch.randn(numel, generator=g) with g a fresh CUDA generator seeded `seed` (Philox offset 0) runs ATen's
+// distribution_elementwise_grid_stride_kernel (ATen/native/cuda/DistributionTemplates.h, torch >= 2.1) with 256-thread blocks,
+//   grid = min(SMs * (max threads per SM / 256), ceil(numel / 256)),  T = 256 * grid threads,  unroll 4:
+// thread idx holds curand_init(seed, idx, 0) and its k-th curand_normal4 (= Philox4x32-10 of counter {k, idx} under key {seed})
+// fills elements li = 4Tk + T*ii + idx, ii = 0..3: Box-Muller of words (w0, w1) for ii 0, 1 and (w2, w3) for ii 2, 3, sin for an
+// even ii and cos for an odd one.  The stream is a function of (seed, numel, SMs, max threads per SM) only.  Draws whose byte
+// extent needs 64-bit indexing are split by ATen into sub-draws with offsets of their own; the library refuses them.
+constexpr int SEED_TORCH_PER_FRAME = 2, SEED_TORCH_PER_CALL = 3;
+constexpr uint32_t TORCH_RANDN_BLOCK = 256;
+
+VRGDG_HD bool torch_stream(int seed_mode) { return seed_mode == SEED_TORCH_PER_FRAME || seed_mode == SEED_TORCH_PER_CALL; }
+
+// T of a draw of numel (>= 1) elements (calc_execution_policy)
+VRGDG_HD uint32_t torch_randn_threads(uint64_t numel, int sms, int max_threads_per_sm) {
+  const uint64_t blocks = (numel + TORCH_RANDN_BLOCK - 1) / TORCH_RANDN_BLOCK;
+  const uint64_t cap = (uint64_t)sms * (uint64_t)(max_threads_per_sm / (int)TORCH_RANDN_BLOCK);
+  return (uint32_t)((blocks < cap ? blocks : cap) * TORCH_RANDN_BLOCK);
+}
+
+// element li of a draw -> (curand4 call k, float4 lane ii, thread idx); li < 2^31 (32-bit indexing)
+struct TorchSite { uint32_t k, ii, idx; };
+VRGDG_HD TorchSite torch_randn_site(uint32_t li, uint32_t T) {
+  TorchSite s;
+  s.k = li / (4u * T);
+  const uint32_t r = li - s.k * (4u * T);
+  s.ii = r / T;
+  s.idx = r - s.ii * T;
+  return s;
+}
+
+// Philox4x32-10 with the key schedule done in place (curand_Philox4x32_10)
+VRGDG_HD U4 philox4x32_10(U4 c, uint32_t k0, uint32_t k1) {
+  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+#pragma unroll
+  for (int r = 0; r < PHILOX_ROUNDS; ++r) {
+    uint32_t h0, l0, h1, l1;
+    mulhilo(M0, c.x, h0, l0);
+    mulhilo(M1, c.z, h1, l1);
+    U4 n;
+    n.x = h1 ^ c.y ^ k0;
+    n.y = l1;
+    n.z = h0 ^ c.w ^ k1;
+    n.w = l0;
+    c = n;
+    k0 += PHILOX_W0;
+    k1 += PHILOX_W1;
+  }
+  return c;
+}
+
+// the 128 bits behind element li: counter {lo k, hi k, lo idx, hi idx}, key {lo seed, hi seed} (k and idx are < 2^32 here)
+VRGDG_HD U4 torch_randn_bits(uint64_t seed, const TorchSite& s) {
+  U4 c;
+  c.x = s.k; c.y = 0u; c.z = s.idx; c.w = 0u;
+  return philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+}
+
+// _curand_box_muller (curand_normal.h) for one output: the same expressions, so nvcc contracts and rounds them the same way
+// (no fast-math, like torch's build); ATen's transform z * 1.0f + 0.0f then turns a -0 (u rounds to 1) into +0.
+VRGDG_HD float torch_box_muller(uint32_t a, uint32_t b, bool cos_lane) {
+  const float u = a * 2.3283064e-10f + (2.3283064e-10f / 2);
+  const float v = b * (2.3283064e-10f * 6.2831855f) + ((2.3283064e-10f * 6.2831855f) / 2);
+  const float s = sqrtf(-2.0f * logf(u));
+  float sn, cs;
+#if defined(__CUDA_ARCH__)
+  __sincosf(v, &sn, &cs);
+#else
+  sn = sinf(v); cs = cosf(v);
+#endif
+  return addx((cos_lane ? cs : sn) * s, 0.0f);
+}
+
+// N(0,1) element li of a draw of T threads (fp32, before any cast to the frame dtype)
+VRGDG_HD float torch_randn(uint64_t seed, uint32_t li, uint32_t T) {
+  const TorchSite s = torch_randn_site(li, T);
+  const U4 w = torch_randn_bits(seed, s);
+  const bool hi = s.ii >= 2;
+  return torch_box_muller(hi ? w.z : w.x, hi ? w.w : w.y, (s.ii & 1u) != 0);
+}
+
+// seed of frame i's draw: PER_FRAME (seed + frame0 + i) & 0x7FFFFFFF (_apply_seeded_grain), PER_CALL the seed itself
+VRGDG_HD uint64_t torch_draw_seed(uint64_t seed, int64_t frame0, int64_t i, int seed_mode) {
+  return seed_mode == SEED_TORCH_PER_FRAME ? ((uint64_t)((int64_t)seed + frame0 + i) & 0x7FFFFFFFull) : seed;
+}
+// index of frame i's first element in its draw: PER_CALL draws [B,H,W,3] at once, PER_FRAME [H,W,3] per frame
+VRGDG_HD uint32_t torch_draw_base(int64_t i, int64_t hw, int seed_mode) {
+  return seed_mode == SEED_TORCH_PER_CALL ? (uint32_t)(i * hw * 3) : 0u;
+}
+
+// the reference's grain mix of channel c (RGB) alone, one rounding per op: s * z'_c + (1 - s) * z_g, z' = (2 z_r, z_g, 3 z_b)
+VRGDG_HD float grain_mix_exact(float zc, float zg, int c, float s, float oms) {
+  const float zs = (c == 0) ? mulx(zc, 2.0f) : ((c == 2) ? mulx(zc, 3.0f) : zc);
+  return addx(mulx(s, zs), mulx(oms, zg));
+}
+
 // ---- grain blend: nodes.py:53-60 ------------------------------------------------------------
 // exact variant = the reference's op sequence, one rounding per op.
 VRGDG_HD void grain_blend_exact(float& r, float& g, float& b, float zr, float zg, float zb,

@@ -30,13 +30,33 @@ def _apply_lut_tensor(image_tensor, lut_name, strength, device):
     return out if str(device) != "cpu" else out.to(image_tensor.device)
 
 
-def _apply_film_grain_tensor(image_tensor, grain_intensity=0.04, saturation_mix=0.5, device="cpu", seed=None):
+NOISE_STREAMS = ("vrgdg", "torch_cuda")
+
+
+def _seed_mode(noise, vrgdg_mode, torch_mode):
+    """`noise` keyword of the grain helpers: "vrgdg" = this package's counter-based generator (the default), "torch_cuda" = torch's
+    CUDA randn stream of the reference's seeded generators, so that seeded grain equals the reference's run on the same GPU model."""
+    if noise == "vrgdg":
+        return vrgdg_mode
+    if noise == "torch_cuda":
+        return torch_mode
+    raise ValueError("vrgdg_b200: noise must be one of %s, got %r" % (NOISE_STREAMS, noise))
+
+
+def _apply_film_grain_tensor(image_tensor, grain_intensity=0.04, saturation_mix=0.5, device="cpu", seed=None, noise="vrgdg"):
+    """noise="torch_cuda": the grain of the reference run on a CUDA tensor with the same seed (one [B,H,W,3] draw of
+    torch.Generator("cuda").manual_seed(seed)).  Unseeded, the reference draws from the global generator's state, which this cannot
+    reproduce: ValueError."""
     intensity = max(0.0, min(1.0, float(grain_intensity)))
     saturation = max(0.0, min(1.0, float(saturation_mix)))
+    mode = _seed_mode(noise, nv.SEED_PER_CLIP, nv.SEED_TORCH_PER_CALL)
+    if seed in (None, "") and mode == nv.SEED_TORCH_PER_CALL:
+        raise ValueError("vrgdg_b200: _apply_film_grain_tensor(noise=\"torch_cuda\") needs a seed: unseeded, the reference draws from "
+                         "torch's global generator state")
     src, dev = _to_cuda(image_tensor, device)
     if seed in (None, ""):
         seed = int(torch.randint(0, 2**62, (1,), dtype=torch.int64).item())
-    out = ops.grain(src, intensity, saturation, 1.0 - saturation, int(seed), frame0=0, seed_mode=nv.SEED_PER_CLIP)
+    out = ops.grain(src, intensity, saturation, 1.0 - saturation, int(seed), frame0=0, seed_mode=mode)
     return out if str(device) != "cpu" else out.to(image_tensor.device)
 
 
@@ -132,18 +152,21 @@ def _apply_unsharp(images, strength, use_gpu):
     return out.to(images.device)
 
 
-def _apply_seeded_grain(images, intensity, saturation_mix, seed, frame_start):
+def _apply_seeded_grain(images, intensity, saturation_mix, seed, frame_start, noise="vrgdg"):
+    """noise="torch_cuda": per frame the CUDA draw of torch.Generator("cuda").manual_seed((seed + frame_start + i) & 0x7FFFFFFF)."""
+    mode = _seed_mode(noise, nv.SEED_PER_FRAME, nv.SEED_TORCH_PER_FRAME)
     if intensity <= 0:
         return images
     src, dev = _to_cuda(images)
     s = float(saturation_mix)
-    out = ops.grain(src, float(intensity), s, 1.0 - s, int(seed), frame0=int(frame_start), seed_mode=nv.SEED_PER_FRAME)
+    out = ops.grain(src, float(intensity), s, 1.0 - s, int(seed), frame0=int(frame_start), seed_mode=mode)
     return out.to(images.device)
 
 
-def _apply_effects_batch(images, settings, frame_start=0):
+def _apply_effects_batch(images, settings, frame_start=0, noise="vrgdg"):
     """unsharp (if enabled) then per-frame seeded grain (if enabled) in ONE fused kernel; returns a CPU tensor like
-    the reference (:294)."""
+    the reference (:294).  noise: as _apply_seeded_grain."""
+    mode = _seed_mode(noise, nv.SEED_PER_FRAME, nv.SEED_TORCH_PER_FRAME)
     use_gpu = bool(settings.get("use_gpu", True))
     src, dev = _to_cuda(images)
     stencil = post = None
@@ -152,30 +175,32 @@ def _apply_effects_batch(images, settings, frame_start=0):
                        border=nv.BORDER_ZERO if use_gpu else nv.BORDER_REPLICATE)
     if settings.get("grain_enabled", False) and float(settings.get("grain_intensity", 0.04)) > 0:
         post = dict(intensity=float(settings.get("grain_intensity", 0.04)), saturation_mix=float(settings.get("saturation_mix", 0.5)),
-                    seed=int(settings.get("seed", 42)), seed_mode=nv.SEED_PER_FRAME)
+                    seed=int(settings.get("seed", 42)), seed_mode=mode)
     if stencil is None and post is None:
         return images.detach().cpu()
     if stencil is None:
         s = post["saturation_mix"]
-        out = ops.grain(src, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start), seed_mode=nv.SEED_PER_FRAME)
+        out = ops.grain(src, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start), seed_mode=mode)
     else:
         out = PostChain(stencil=stencil, post_grain=post, device=dev)(src, first_frame=int(frame_start))
     return out.detach().cpu()
 
 
-def enhance_frames(frames, output_width, output_height, settings, frame_start=0):
+def enhance_frames(frames, output_width, output_height, settings, frame_start=0, noise="vrgdg"):
     """The data path of one batch of the standalone enhancer's render loop (EnhancerNodes.py:415-420):
     `_tensor_to_frames(_apply_effects_batch(_frames_to_tensor(_resize_frames(frames, w, h)), settings, frame_start))`, bytes in ->
     bytes out, without leaving the GPU in between: one upload of the decoded uint8 BGR frames, Lanczos4 resize (2 launches, only if
     the size differs), unsharp + per-frame seeded grain directly on the bytes (1 launch), one download.  Byte-identical to the
-    four helpers called one after the other."""
+    four helpers called one after the other.  noise: as _apply_seeded_grain ("torch_cuda" = the reference's frames on a CUDA device)."""
+    mode = _seed_mode(noise, nv.SEED_PER_FRAME, nv.SEED_TORCH_PER_FRAME)
     output_width, output_height = max(1, int(output_width)), max(1, int(output_height))
     if not frames:
         return []
     shapes = {tuple(f.shape) for f in frames}
     if len(shapes) != 1 or len(next(iter(shapes))) != 3 or next(iter(shapes))[2] != 3 or any(f.dtype != np.uint8 for f in frames):
         # mixed sizes are legal for the reference (cv2 resizes frame by frame): take the helper-by-helper route
-        return _tensor_to_frames(_apply_effects_batch(_frames_to_tensor(_resize_frames(frames, output_width, output_height)), settings, frame_start))
+        return _tensor_to_frames(_apply_effects_batch(_frames_to_tensor(_resize_frames(frames, output_width, output_height)), settings, frame_start,
+                                                      noise=noise))
     dev = compute_device()
     batch = upload(torch.from_numpy(np.stack([np.ascontiguousarray(f) for f in frames], axis=0)), dev)
     if batch.shape[1] != output_height or batch.shape[2] != output_width:
@@ -187,12 +212,12 @@ def enhance_frames(frames, output_width, output_height, settings, frame_start=0)
                        border=nv.BORDER_ZERO if use_gpu else nv.BORDER_REPLICATE)
     if settings.get("grain_enabled", False) and float(settings.get("grain_intensity", 0.04)) > 0:
         post = dict(intensity=float(settings.get("grain_intensity", 0.04)), saturation_mix=float(settings.get("saturation_mix", 0.5)),
-                    seed=int(settings.get("seed", 42)), seed_mode=nv.SEED_PER_FRAME)
+                    seed=int(settings.get("seed", 42)), seed_mode=mode)
     if stencil is not None:
         batch = PostChain(stencil=stencil, post_grain=post, device=dev)(batch, first_frame=int(frame_start))
     elif post is not None:
         s = post["saturation_mix"]
-        batch = ops.grain(batch, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start), seed_mode=nv.SEED_PER_FRAME)
+        batch = ops.grain(batch, post["intensity"], s, 1.0 - s, post["seed"], frame0=int(frame_start), seed_mode=mode)
     return list(batch.cpu().numpy())
 
 

@@ -68,8 +68,30 @@ enum { VRGDG_BORDER_REPLICATE = 0, VRGDG_BORDER_ZERO = 1 };
  *              (FastFilmGrain nodes.py:51, _apply_film_grain_tensor VRGDG_LUTVideoTools.py:268-272)
  *   PER_FRAME: key = (seed + frame0 + i) & 0x7FFFFFFF, frame counter = 0
  *              (_apply_seeded_grain VRGDG_StandaloneVideoEnhancerNodes.py:266-269)
- * Both make the result independent of batch boundaries and of how frames are sharded. */
-enum { VRGDG_SEED_PER_CLIP = 0, VRGDG_SEED_PER_FRAME = 1 };
+ * Both make the result independent of batch boundaries and of how frames are sharded.
+ *
+ * The two torch-stream modes reproduce, bit for bit, the N(0,1) tensor torch.randn draws on the CURRENT CUDA device from a fresh
+ * torch.Generator("cuda") seeded s (torch >= 2.1, float32 / float16 / bfloat16 draws), so seeded grain equals the reference's:
+ *   TORCH_PER_FRAME: one draw of [H,W,3] per frame, s = (seed + frame0 + i) & 0x7FFFFFFF
+ *                    (_apply_seeded_grain VRGDG_StandaloneVideoEnhancerNodes.py:261-275 on a CUDA device)
+ *   TORCH_PER_CALL : one draw of [B,H,W,3] for the whole call, s = seed (manual_seed's 64-bit value; frame0 is not used)
+ *                    (_apply_film_grain_tensor VRGDG_LUTVideoTools.py:262-277 on a CUDA tensor)
+ * The stream (ATen/native/cuda/DistributionTemplates.h: calc_execution_policy, distribution_elementwise_grid_stride_kernel,
+ * normal_kernel; curand_kernel.h / curand_normal.h): for a draw of n elements,
+ *   T = 256 * min(SMs * (max threads per SM / 256), ceil(n / 256))       (132 * 8 blocks on an H100 SXM: T = 270336)
+ *   element li: k = li / 4T, ii = (li mod 4T) / T, idx = li mod T
+ *   (w0,w1,w2,w3) = Philox4x32-10(counter {lo k, hi k, lo idx, hi idx}, key {lo s, hi s})  = the k-th curand4 of curand_init(s, idx, 0)
+ *   Box-Muller of (w0,w1) for ii 0,1 and (w2,w3) for ii 2,3 as _curand_box_muller: u = a 2^-32 + 2^-33, v = (b 2^-32 + 2^-33) 2 pi,
+ *   sqrtf(-2 logf(u)) times __sinf(v) for an even ii, __cosf(v) for an odd one; then z * 1 + 0 (a -0 becomes +0) and the cast to the
+ *   frame dtype (round to nearest) on 16-bit frames.  uint8 frames use a float32 draw, as the reference's byte path does.
+ * Pixel p's channels are elements 3p + c in RGB order (uint8 BGR frames included).  SMs and max threads per SM are read from the
+ * current device: the stream is the reference's on the same GPU model, and shards on cards with other SM counts draw their own
+ * card's stream.  Torch-stream grain always runs the reference's op order with one rounding per op (mix, multiply, add, clamp).
+ * Accepted by vrgdg_grain and vrgdg_grain_noise (both modes) and by the chain's post-grain stage (TORCH_PER_FRAME only).
+ * VRGDG_E_UNSUPPORTED, before any CUDA call: a torch mode in the chain's first grain stage (the reference's FastFilmGrain draws
+ * from the global generator), TORCH_PER_CALL for post grain, and a draw whose byte extent 1 + (n - 1) * element size exceeds
+ * INT32_MAX (torch splits such a draw into sub-draws with Philox offsets of their own). */
+enum { VRGDG_SEED_PER_CLIP = 0, VRGDG_SEED_PER_FRAME = 1, VRGDG_SEED_TORCH_PER_FRAME = 2, VRGDG_SEED_TORCH_PER_CALL = 3 };
 enum { VRGDG_RESIZE_NEAREST = 0, VRGDG_RESIZE_BILINEAR = 1, VRGDG_RESIZE_BICUBIC = 2, VRGDG_RESIZE_AREA = 3 };
 
 /* ---- library ---------------------------------------------------------------------------- */
@@ -335,7 +357,8 @@ VRGDG_API int vrgdg_lanczos4_resize_u8(const uint8_t* in, uint8_t* out, int B, i
 VRGDG_API int vrgdg_u8bgr_to_rgb(const uint8_t* in, void* out, int64_t npix, int dtype, void* stream);
 VRGDG_API int vrgdg_rgb_to_u8bgr(const void* in, uint8_t* out, int64_t npix, int dtype, void* stream);
 
-/* Raw N(0,1) stream of the grain generator ([B,H,W,3] fp32), for distribution tests. */
+/* Raw N(0,1) stream of the grain generator ([B,H,W,3] fp32), for distribution tests.  Torch-stream modes give the draw before any
+ * cast (fp32): a 16-bit draw of the reference is this output rounded to nearest. */
 VRGDG_API int vrgdg_grain_noise(float* out, int B, int H, int W, uint64_t seed, int64_t frame0,
                       int seed_mode, void* stream);
 
