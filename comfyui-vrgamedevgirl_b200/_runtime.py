@@ -70,6 +70,19 @@ def devices_from_env():
     return [torch.device("cuda", i) for i in idx]
 
 
+# noise sources of the grain: "vrgdg" = this package's counter-based generator, "torch_cuda" = torch's CUDA randn stream
+NOISE_STREAMS = ("vrgdg", "torch_cuda")
+
+
+def grain_noise_from_env():
+    """FastFilmGrain's noise source, VRGDG_GRAIN_NOISE: unset, empty or "vrgdg" = this package's generator (the default);
+    "torch_cuda" = the draws the reference makes from the compute device's global CUDA generator.  Read at call time."""
+    raw = os.environ.get("VRGDG_GRAIN_NOISE", "").strip()
+    if raw in ("",) + NOISE_STREAMS:
+        return raw or NOISE_STREAMS[0]
+    raise ValueError("VRGDG_GRAIN_NOISE=%s: use one of %s" % (raw, " or ".join(NOISE_STREAMS)))
+
+
 def result_device(images, numpy_path=False):
     """Where a node returns its IMAGE.  Inside ComfyUI: exactly what the reference does
     (intermediate_device() nodes.py:65,123,177; CPU for the numpy paths :209).  Outside: the input's device."""

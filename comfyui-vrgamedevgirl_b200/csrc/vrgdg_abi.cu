@@ -312,6 +312,51 @@ int vrgdg_grain(const void* in, void* out, int B, int H, int W, int dtype, float
   return VRGDG_OK;
 }
 
+int vrgdg_grain_torch_global(const void* in, void* out, int B, int H, int W, int dtype, float intensity, float sat, float one_minus_sat,
+                             uint64_t seed, uint64_t philox_offset, int64_t frame0, int64_t clip_frames, int64_t draw_frames,
+                             void* stream) {
+  const char* who = "vrgdg_grain_torch_global";
+  int rc = check_frames(in, out, B, H, W, dtype, who);
+  if (rc) return rc;
+  if (dtype == VRGDG_U8BGR) return fail(VRGDG_E_UNSUPPORTED, "%s: takes float frames (IMAGE tensors); uint8 frames are not drawn this way", who);
+  if (philox_offset % 4) return fail(VRGDG_E_INVALID, "%s: Philox offset %llu is not a multiple of 4", who, (unsigned long long)philox_offset);
+  if (draw_frames < 1) return fail(VRGDG_E_INVALID, "%s: draw_frames %lld < 1", who, (long long)draw_frames);
+  if (clip_frames > INT32_MAX || frame0 < 0 || frame0 > clip_frames - B)
+    return fail(VRGDG_E_INVALID, "%s: frames [%lld, %lld) do not lie in a clip of %lld frames", who, (long long)frame0,
+                (long long)(frame0 + B), (long long)clip_frames);
+  if ((int64_t)B * H * W == 0) return VRGDG_OK;
+  const int64_t n = (int64_t)H * W * 3, step = draw_frames < clip_frames ? draw_frames : clip_frames;
+  // every draw fits when the first (full) one does; checking one frame first keeps step * n from overflowing
+  if ((rc = check_torch_draw(n, torch_draw_es(dtype), who)) || (rc = check_torch_draw(step * n, torch_draw_es(dtype), who))) return rc;
+  LaunchCtx ctx;
+  if ((rc = get_ctx(stream, ctx))) return rc;
+  PointParams P;
+  zero_point(P, B, H, W);
+  P.gI = intensity; P.gs = sat; P.goms = one_minus_sat;
+  P.seed = seed; P.frame0 = frame0; P.seed_mode = SEED_TORCH_GLOBAL;
+  // every index below is 32-bit now: clip_frames <= INT32_MAX and step * n <= INT32_MAX
+  P.toffset = philox_offset; P.tstep = (uint32_t)step; P.tclip = (uint32_t)clip_frames;
+  P.tT = torch_randn_threads((uint64_t)(step * n), ctx.sms, ctx.threads_per_sm);
+  const uint32_t last = torch_global_draw(P.tclip - 1, P.tstep);
+  P.tT_last = torch_randn_threads(torch_global_numel(last, P.tstep, P.tclip, (uint32_t)n), ctx.sms, ctx.threads_per_sm);
+#define PT(T) launch_point<T>(in, out, P, ST_GRAIN, true, ctx)
+  cudaError_t e = DISPATCH_DTYPE(dtype, PT);
+#undef PT
+  if (e != cudaSuccess) return fail_cuda(e, who);
+  return VRGDG_OK;
+}
+
+int vrgdg_torch_randn_increment(int64_t numel, int64_t* inc) {
+  if (!inc) return fail(VRGDG_E_INVALID, "vrgdg_torch_randn_increment: null output");
+  if (numel < 0) return fail(VRGDG_E_INVALID, "vrgdg_torch_randn_increment: negative numel %lld", (long long)numel);
+  if (numel == 0) { *inc = 0; return VRGDG_OK; }
+  LaunchCtx ctx;
+  int rc = get_ctx(nullptr, ctx);
+  if (rc) return rc;
+  *inc = (int64_t)torch_randn_increment((uint64_t)numel, torch_randn_threads((uint64_t)numel, ctx.sms, ctx.threads_per_sm));
+  return VRGDG_OK;
+}
+
 int vrgdg_grain_noise(float* out, int B, int H, int W, uint64_t seed, int64_t frame0, int seed_mode, void* stream) {
   if (B < 0 || H < 0 || W < 0) return fail(VRGDG_E_INVALID, "vrgdg_grain_noise: negative shape");
   if ((int64_t)B * H * W == 0) return VRGDG_OK;

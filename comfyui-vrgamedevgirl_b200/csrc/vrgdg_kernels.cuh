@@ -67,8 +67,8 @@ template <> __device__ __forceinline__ float noise_ld<float>(float v) { return v
 
 // element li of a torch-stream draw as the reference's noise tensor holds it: cast to the frame dtype (round to nearest) for 16-bit
 // frames, fp32 for fp32 and uint8 frames (the reference's byte path works on fp32 tensors)
-template <typename T> __device__ __forceinline__ float torch_noise(uint64_t seed, uint32_t li, uint32_t nT) {
-  const float z = torch_randn(seed, li, nT);
+template <typename T> __device__ __forceinline__ float torch_noise(uint64_t seed, uint32_t li, uint32_t nT, uint64_t off4 = 0) {
+  const float z = torch_randn(seed, li, nT, off4);
   return sizeof(T) == 2 ? Elem<T>::ld(Elem<T>::st(z)) : z;
 }
 
@@ -82,7 +82,10 @@ struct PointParams {
   int64_t frame0;
   int seed_mode;
   GrainKey gkey;               // Philox round keys, evaluated on the host
-  uint32_t tT;                 // torch-stream modes: threads T of each draw (torch_randn_threads)
+  uint32_t tT;                 // torch-stream modes: threads T of each draw (torch_randn_threads); SEED_TORCH_GLOBAL: of a full draw
+  // SEED_TORCH_GLOBAL: Philox offset o0 of the first draw, frames per draw, frames of the clip, threads T of the last draw
+  uint64_t toffset;
+  uint32_t tstep, tclip, tT_last;
   const void* ext_noise;       // [B,H,W,3] of the frame dtype, or null
   // colour match
   const float* cm_params;      // [B][12]
@@ -90,6 +93,18 @@ struct PointParams {
   // LUT
   LutParams lut;
 };
+
+// SEED_TORCH_GLOBAL: the draw batch frame `frame` lies in, as its Philox block offset, threads T and the index of the frame's first
+// element in it
+struct TorchDraw { uint64_t off4; uint32_t T, base; };
+__device__ __forceinline__ TorchDraw torch_global_frame_draw(const PointParams& P, int frame) {
+  const uint32_t f = (uint32_t)P.frame0 + (uint32_t)frame, n = (uint32_t)P.hw * 3u, j = torch_global_draw(f, P.tstep);
+  TorchDraw d;
+  d.off4 = torch_global_offset(P.toffset, j, P.tstep, n, P.tT) >> 2;
+  d.T = torch_global_threads(j, P.tstep, P.tclip, P.tT, P.tT_last);
+  d.base = torch_global_base(f, P.tstep, n);
+  return d;
+}
 
 // One pixel through the enabled stages; (zr,zg,zb) = this pixel's N(0,1) triple (generator or external).
 template <int MASK, bool EXACT>
@@ -156,7 +171,8 @@ k_point(const T* __restrict__ in, T* __restrict__ out, PointParams P,
   constexpr int NE = PX * 3;
   constexpr bool GRAIN = (MASK & ST_GRAIN) != 0;
   const bool has_ext = GRAIN && (P.ext_noise != nullptr);
-  const bool tstream = EXACT && GRAIN && torch_stream(P.seed_mode);   // torch's randn stream: exact blend only (host-enforced)
+  // torch's randn stream, of fresh generators or of the global one: exact blend only (host-enforced)
+  const bool tstream = EXACT && GRAIN && (torch_stream(P.seed_mode) || P.seed_mode == SEED_TORCH_GLOBAL);
   for (int64_t vb = blockIdx.x; vb < total_vblocks; vb += gridDim.x) {
     const int frame = (int)(vb / blocks_per_frame);
     const int bif = (int)(vb - (int64_t)frame * blocks_per_frame);
@@ -195,6 +211,18 @@ k_point(const T* __restrict__ in, T* __restrict__ out, PointParams P,
       } else {
 #pragma unroll
         for (int i = 0; i < NE; ++i) nz[i] = noise_ld<noise_t>(ns[i]);
+      }
+    } else if (tstream && P.seed_mode == SEED_TORCH_GLOBAL) {
+      // one element per iteration, the loop kept rolled: unrolled like the branch below, this mode's 64-bit counter offset raised the
+      // register count of the exact grain kernels that every torch-stream mode and ext_noise share, and made grain + LUT spill
+      const TorchDraw d = torch_global_frame_draw(P, frame);
+      const uint32_t li0 = d.base + (uint32_t)pix0 * 3u;
+#pragma unroll 1
+      for (int i = 0; i < NE; ++i) {
+        const float z = torch_noise<T>(P.seed, li0 + (uint32_t)i, d.T, d.off4);
+#pragma unroll
+        for (int m = 0; m < NE; ++m)
+          if (m == i) nz[m] = z;
       }
     } else if (tstream) {   // the PX pixels lie in one frame: consecutive elements of its draw, RGB order
       const uint64_t dseed = torch_draw_seed(P.seed, P.frame0, frame, P.seed_mode);

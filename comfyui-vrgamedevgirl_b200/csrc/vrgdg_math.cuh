@@ -247,10 +247,14 @@ VRGDG_HD U4 philox4x32_10(U4 c, uint32_t k0, uint32_t k1) {
   return c;
 }
 
-// the 128 bits behind element li: counter {lo k, hi k, lo idx, hi idx}, key {lo seed, hi seed} (k and idx are < 2^32 here)
-VRGDG_HD U4 torch_randn_bits(uint64_t seed, const TorchSite& s) {
+// the 128 bits behind element li: counter {lo k', hi k', lo idx, hi idx}, key {lo seed, hi seed}, k' = k + off4 in 64 bits.
+// off4 = Philox offset / 4: curand_init(seed, idx, offset) skips offset / 4 whole Philox blocks (ATen's offsets are multiples of
+// 4), so the addition may carry into the second counter word.  Fresh generators (the per-frame / per-call modes) have off4 = 0.
+// k < 2^31 and off4 < 2^62, so k' never carries into the idx words.
+VRGDG_HD U4 torch_randn_bits(uint64_t seed, const TorchSite& s, uint64_t off4 = 0) {
+  const uint64_t k = (uint64_t)s.k + off4;
   U4 c;
-  c.x = s.k; c.y = 0u; c.z = s.idx; c.w = 0u;
+  c.x = (uint32_t)k; c.y = (uint32_t)(k >> 32); c.z = s.idx; c.w = 0u;
   return philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
 }
 
@@ -269,10 +273,10 @@ VRGDG_HD float torch_box_muller(uint32_t a, uint32_t b, bool cos_lane) {
   return addx((cos_lane ? cs : sn) * s, 0.0f);
 }
 
-// N(0,1) element li of a draw of T threads (fp32, before any cast to the frame dtype)
-VRGDG_HD float torch_randn(uint64_t seed, uint32_t li, uint32_t T) {
+// N(0,1) element li of a draw of T threads at Philox block offset off4 (fp32, before any cast to the frame dtype)
+VRGDG_HD float torch_randn(uint64_t seed, uint32_t li, uint32_t T, uint64_t off4 = 0) {
   const TorchSite s = torch_randn_site(li, T);
-  const U4 w = torch_randn_bits(seed, s);
+  const U4 w = torch_randn_bits(seed, s, off4);
   const bool hi = s.ii >= 2;
   return torch_box_muller(hi ? w.z : w.x, hi ? w.w : w.y, (s.ii & 1u) != 0);
 }
@@ -284,6 +288,43 @@ VRGDG_HD uint64_t torch_draw_seed(uint64_t seed, int64_t frame0, int64_t i, int 
 // index of frame i's first element in its draw: PER_CALL draws [B,H,W,3] at once, PER_FRAME [H,W,3] per frame
 VRGDG_HD uint32_t torch_draw_base(int64_t i, int64_t hw, int seed_mode) {
   return seed_mode == SEED_TORCH_PER_CALL ? (uint32_t)(i * hw * 3) : 0u;
+}
+
+// ---- the global generator's stream (library-internal mode SEED_TORCH_GLOBAL, vrgdg_grain_torch_global) -------------------
+// FastFilmGrain (nodes.py:41-66) calls torch.randn_like once per mini-batch of `step` frames on the device's default CUDA generator
+// (seed s, Philox offset o0 before the call).  Draw j holds frames [j step, min((j+1) step, clip)), numel_j = frames_j * n elements
+// (n = H W 3), and starts at offset o_j = o0 + sum_{i<j} inc(numel_i) = o0 + j inc(step n): every draw but the last is full.
+// Everything is a function of the absolute frame index, so chunks and shards need nothing extra.  The library takes clips of at
+// most INT32_MAX frames and draws of at most INT32_MAX elements (32-bit indexing), so frame and element indices are 32-bit here:
+// the kernels divide in 32 bits.
+constexpr int SEED_TORCH_GLOBAL = 4;   // not a public seed mode: vrgdg_grain refuses it
+
+// Philox offset a draw of numel elements on T threads consumes (calc_execution_policy's counter_offset: 4 curand calls per unrolled
+// iteration; philox_cuda_state rounds it to a multiple of 4, which it already is).  ATen returns before drawing an empty tensor.
+template <typename I>
+VRGDG_HD I torch_randn_increment(I numel, uint32_t T) {
+  return numel == 0 ? (I)0 : ((numel - 1) / ((I)4 * T) + 1) * (I)4;
+}
+
+// draw index of absolute frame f, and the index of its first element in that draw
+VRGDG_HD uint32_t torch_global_draw(uint32_t f, uint32_t step) { return f / step; }
+VRGDG_HD uint32_t torch_global_base(uint32_t f, uint32_t step, uint32_t n) { return (f - (f / step) * step) * n; }
+
+// elements of draw j of a clip of `clip` frames; only the last draw can hold fewer than step frames
+VRGDG_HD uint32_t torch_global_numel(uint32_t j, uint32_t step, uint32_t clip, uint32_t n) {
+  const uint32_t left = clip - j * step;   // frames from the draw's first one to the end of the clip
+  return (left < step ? left : step) * n;
+}
+VRGDG_HD bool torch_global_is_last(uint32_t j, uint32_t step, uint32_t clip) { return clip - j * step <= step; }
+
+// T of draw j, given T of a full draw and of the last one (torch_randn_threads of their numel, read on the launching device)
+VRGDG_HD uint32_t torch_global_threads(uint32_t j, uint32_t step, uint32_t clip, uint32_t T_full, uint32_t T_last) {
+  return torch_global_is_last(j, step, clip) ? T_last : T_full;
+}
+
+// Philox offset o_j of draw j (64-bit, wrapping as the generator's own uint64 offset does)
+VRGDG_HD uint64_t torch_global_offset(uint64_t o0, uint32_t j, uint32_t step, uint32_t n, uint32_t T_full) {
+  return o0 + (uint64_t)j * torch_randn_increment<uint32_t>(step * n, T_full);
 }
 
 // the reference's grain mix of channel c (RGB) alone, one rounding per op: s * z'_c + (1 - s) * z_g, z' = (2 z_r, z_g, 3 z_b)

@@ -10,7 +10,7 @@ import torch
 
 from . import _native as nv
 from . import ops
-from ._runtime import compute_device, devices_from_env, result_device, run_frames, upload
+from ._runtime import compute_device, cuda_device, devices_from_env, grain_noise_from_env, result_device, run_frames, upload
 
 _FLOATS = (torch.float32, torch.float16, torch.bfloat16)
 
@@ -50,6 +50,8 @@ class FastFilmGrain:
 
     def apply_grain(self, images, grain_intensity, saturation_mix, batch_size):
         images = _as_frames(images)
+        if grain_noise_from_env() == "torch_cuda":
+            return (_global_stream_grain(images, grain_intensity, float(saturation_mix), batch_size),)
         seed = draw_seed()
         sat = float(saturation_mix)
         # batch_size only bounds device memory while streaming host frames; the noise is keyed by the absolute
@@ -59,6 +61,34 @@ class FastFilmGrain:
         devs = devices_from_env() if images.device.type == "cpu" else None
         out = run_frames(images, lambda dev: run, batch_size, result_device(images), compute_device(images), devs)
         return (out,)
+
+
+def _global_stream_grain(images, intensity, sat, batch_size):
+    """FastFilmGrain with VRGDG_GRAIN_NOISE=torch_cuda: the noise the reference draws on a CUDA device, torch.randn_like once per
+    mini-batch of batch_size frames (0 = the whole batch) from the compute device's global generator, and that generator advanced
+    as those draws advance it.  Unlike the default path, the grain here depends on batch_size, as the reference's does.  The
+    CPU generator is not touched (the reference does not touch it either)."""
+    B, H, W = (int(s) for s in images.shape[:3])
+    step = min(int(batch_size), B) if int(batch_size) > 0 else B            # nodes.py:46; one draw when batch_size >= B
+    n = H * W * 3
+    if B > 0 and n > 0 and 1 + (step * n - 1) * images.element_size() > 2**31 - 1:
+        raise ValueError("vrgdg_b200: FastFilmGrain with VRGDG_GRAIN_NOISE=torch_cuda: a draw of %d frames of %dx%d (batch_size=%d) "
+                         "exceeds 32-bit indexing (torch splits such a draw into sub-draws, which is not reproduced); lower batch_size"
+                         % (step, W, H, int(batch_size)))
+    dev = cuda_device(compute_device(images))
+    torch.cuda.init()
+    gen = torch.cuda.default_generators[dev.index]
+    seed, offset = gen.initial_seed(), gen.get_offset()
+    total = 0
+    if B > 0 and n > 0:
+        total = (B // step) * ops.torch_randn_increment(step * n, dev) + ops.torch_randn_increment((B % step) * n, dev)
+
+    def run(frames, first):
+        return ops.grain_torch_global(frames, intensity, sat, 1.0 - sat, seed, offset, first, B, step)
+    devs = devices_from_env() if images.device.type == "cpu" else None
+    out = run_frames(images, lambda card: run, batch_size, result_device(images), dev, devs)
+    gen.set_offset(offset + total)
+    return out
 
 
 class ColorMatchToReference:

@@ -91,6 +91,30 @@ def grain(images, intensity, sat, one_minus_sat, seed, frame0=0, seed_mode=nv.SE
     return out
 
 
+def grain_torch_global(images, intensity, sat, one_minus_sat, seed, philox_offset, frame0, clip_frames, draw_frames):
+    """Frames [frame0, frame0 + B) of a clip of clip_frames frames with FastFilmGrain's grain drawn from a CUDA generator of seed `seed`
+    at Philox offset `philox_offset`, one draw per `draw_frames` frames of the clip (vrgdg_grain_torch_global).  The generator is
+    not advanced here."""
+    t = _frames(images)
+    out = torch.empty_like(t)
+    B, H, W, _ = t.shape
+    lib = nv.load_library()
+    with torch.cuda.device(t.device):
+        nv.check(lib.vrgdg_grain_torch_global(nv.ptr(t), nv.ptr(out), B, H, W, nv.DTYPE_CODE[t.dtype], _f32(intensity), _f32(sat),
+                                              _f32(one_minus_sat), ctypes.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF),
+                                              ctypes.c_uint64(int(philox_offset) & 0xFFFFFFFFFFFFFFFF), ctypes.c_int64(int(frame0)),
+                                              ctypes.c_int64(int(clip_frames)), ctypes.c_int64(int(draw_frames)), nv.stream_ptr(t.device)))
+    return out
+
+
+def torch_randn_increment(numel, device):
+    """The Philox offset torch.randn of `numel` elements consumes on `device`'s CUDA generator (vrgdg_torch_randn_increment)."""
+    inc = ctypes.c_int64(0)
+    with torch.cuda.device(device):
+        nv.check(nv.load_library().vrgdg_torch_randn_increment(ctypes.c_int64(int(numel)), ctypes.byref(inc)))
+    return int(inc.value)
+
+
 def grain_noise(B, H, W, seed, frame0=0, seed_mode=nv.SEED_PER_CLIP, device="cuda"):
     out = torch.empty((B, H, W, 3), dtype=torch.float32, device=device)
     lib = nv.load_library()

@@ -11,7 +11,7 @@ import torch
 
 from . import _native as nv
 from . import ops
-from ._runtime import compute_device, upload
+from ._runtime import NOISE_STREAMS, compute_device, upload
 from .chain import PostChain
 from .lut_nodes import VRGDG_LUTS, _run_lut
 
@@ -28,9 +28,6 @@ def _apply_lut_tensor(image_tensor, lut_name, strength, device):
     src, dev = _to_cuda(image_tensor, device)
     out = _run_lut(src, lut_data, strength)
     return out if str(device) != "cpu" else out.to(image_tensor.device)
-
-
-NOISE_STREAMS = ("vrgdg", "torch_cuda")
 
 
 def _seed_mode(noise, vrgdg_mode, torch_mode):

@@ -138,6 +138,33 @@ VRGDG_API int vrgdg_grain(const void* in, void* out, int B, int H, int W, int dt
                 uint64_t seed, int64_t frame0, int seed_mode,
                 const void* ext_noise, void* stream);
 
+/* FastFilmGrain's grain from the device's global CUDA generator, as the reference draws it: torch.randn_like once per mini-batch
+ * of `draw_frames` frames of the clip (nodes.py:41-66 on a CUDA device), then the reference's op order with one rounding per op.
+ * seed = the generator's initial_seed(), philox_offset = its get_offset() before the call (a multiple of 4).  The call covers
+ * frames [frame0, frame0 + B) of a clip of clip_frames frames (frame0 + B <= clip_frames <= INT32_MAX); draw_frames >= 1
+ * (a value above clip_frames acts as clip_frames: one draw).  With n = H W 3 and step = draw_frames:
+ *   draw j holds frames [j step, min((j+1) step, clip_frames)): numel_j = frames_j * n elements, drawn in the frame dtype;
+ *   inc(numel) = ((numel - 1) / 4T + 1) * 4 with T = 256 * min(SMs * (max threads per SM / 256), ceil(numel / 256)) of the
+ *     current device (calc_execution_policy; vrgdg_torch_randn_increment returns it);
+ *   draw j starts at Philox offset o_j = philox_offset + sum_{i<j} inc(numel_i) = philox_offset + j inc(step n);
+ *   element li of draw j is the stream of the torch-stream modes above with T = T_j and counter
+ *     {lo(k + o_j/4), hi(k + o_j/4), lo idx, hi idx} (64-bit addition) = the k-th curand4 of curand_init(seed, idx, o_j);
+ *   frame f is draw f / step from element (f mod step) n on.
+ * The grain is a function of the absolute frame index, so the clip may be cut into calls (and shards) anywhere.  The library
+ * neither reads nor advances the generator: the caller sets its offset to philox_offset + sum_j inc(numel_j) afterwards, as the
+ * reference's draws leave it.  Float dtypes only (IMAGE tensors): uint8 frames -> VRGDG_E_UNSUPPORTED.  A draw whose byte extent
+ * 1 + (numel_j - 1) * element size exceeds INT32_MAX -> VRGDG_E_UNSUPPORTED ("exceeds 32-bit indexing"; torch splits it into
+ * sub-draws); both are refused before any CUDA call.  SMs are those of the current device: cards of other SM counts draw their
+ * own card's stream. */
+VRGDG_API int vrgdg_grain_torch_global(const void* in, void* out, int B, int H, int W, int dtype,
+                             float intensity, float sat, float one_minus_sat,
+                             uint64_t seed, uint64_t philox_offset, int64_t frame0, int64_t clip_frames, int64_t draw_frames,
+                             void* stream);
+
+/* *inc = the Philox offset torch.randn of numel elements consumes on the current device's CUDA generator: inc(numel) above
+ * (0 for numel 0, without a CUDA call). */
+VRGDG_API int vrgdg_torch_randn_increment(int64_t numel, int64_t* inc);
+
 /* ---- 3x3 stencil sharpeners --------------------------------------------------------------------
  * Replaces FastUnsharpSharpen / FastLaplacianSharpen / FastSobelSharpen (nodes.py:156-384) and
  * _apply_unsharp (VRGDG_StandaloneVideoEnhancerNodes.py:233-258).  TMA-tiled when rows are 16-byte
