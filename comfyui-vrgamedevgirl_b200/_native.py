@@ -105,6 +105,7 @@ SIGNATURES = {
     "vrgdg_lut3d_apply": (_i, [_vp, _vp, _i64, _i, _i, _vp, _i, _fp, _fp, _f, _f, _vp]),
     "vrgdg_grain": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _u64, _i64, _i, _vp, _vp]),
     "vrgdg_grain_torch_global": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _u64, _u64, _i64, _i64, _i64, _vp]),
+    "vrgdg_grain_noise_torch_global": (_i, [_vp, _i, _i, _i, _i, _u64, _u64, _i64, _i64, _i64, _vp]),
     "vrgdg_torch_randn_increment": (_i, [_i64, ctypes.POINTER(_i64)]),
     "vrgdg_grain_noise": (_i, [_vp, _i, _i, _i, _u64, _i64, _i, _vp]),
     "vrgdg_stencil3x3": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp]),

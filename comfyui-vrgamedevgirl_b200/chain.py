@@ -12,7 +12,7 @@ import torch
 
 from . import _native as nv
 from . import ops
-from ._runtime import compute_device, cuda_device, stream_frames, stream_frames_sharded, upload
+from ._runtime import compute_device, cuda_device, pipeline_chunk, stream_frames, stream_frames_sharded, upload
 
 
 class PostChain:
@@ -20,6 +20,10 @@ class PostChain:
         """
         grain / post_grain: dict(intensity, saturation_mix, seed, seed_mode=SEED_PER_CLIP); post_grain also takes
                             seed_mode=SEED_TORCH_PER_FRAME (torch's CUDA randn stream of the enhancer's per-frame seeded generators)
+        grain may instead carry torch_global=dict(seed, philox_offset, clip_frames, draw_frames): a snapshot of a global CUDA
+                            generator (filter_nodes.GlobalStreamDraws), so that the grain is FastFilmGrain's under
+                            VRGDG_GRAIN_NOISE=torch_cuda: one randn_like per draw_frames frames of a clip of clip_frames frames.
+                            The chain neither reads nor advances a generator; the frames' first_frame keys the draws.
         colormatch:         dict(reference_image=[1,H,W,3] tensor  |  ref_sums=[1,7] float64, strength)
         lut:                dict(lut_data={"lut","domain_min","domain_max"}, strength 0..10)
         stencil:            dict(op=STENCIL_*, strength, border=BORDER_REPLICATE)
@@ -145,6 +149,18 @@ class PostChain:
             raise ValueError("vrgdg_b200: PostChain stencil op %d (a torch conv2d path) takes 3-channel frames, got 4 channels"
                              % self.stencil["op"])
 
+    def _torch_global(self, frames, ext_noise):
+        """the grain's global-stream snapshot, or None; ValueError for what that stream cannot grain (uint8 frames, whose draws the
+        reference makes from fp32 tensors, and a caller's ext_noise, which would replace the stream)"""
+        tg = self.grain.get("torch_global") if self.grain is not None else None
+        if tg is None:
+            return None
+        if ext_noise is not None:
+            raise ValueError("vrgdg_b200: PostChain grain with torch_global draws its own noise; ext_noise cannot replace it")
+        if isinstance(frames, torch.Tensor) and frames.dtype == torch.uint8:
+            raise ValueError("vrgdg_b200: PostChain grain with torch_global takes float frames (IMAGE tensors), got uint8")
+        return tg
+
     def __call__(self, frames, first_frame=0, ext_noise=None, out=None, fast_math=False):
         """frames: CUDA [B,H,W,3], or [B,H,W,4] with only `lut` / `stencil` set (check_frames); first_frame: absolute index of
         frames[0] in the clip (keys the grain).  ext_noise (tests): N(0,1) tensor replacing the generator; fast_math then selects the
@@ -154,6 +170,26 @@ class PostChain:
     def _run(self, frames, first_frame, worker, ext_noise=None, out=None, fast_math=False):
         """__call__ with the colour-match scratch of `worker` (the index of a stream_frames_sharded worker on the frames' device)."""
         self.check_frames(frames)
+        tg = self._torch_global(frames, ext_noise)
+        if tg is None:
+            return self._apply(frames, first_frame, worker, ext_noise, out, fast_math)
+        # the global stream's noise, materialised for at most one pipeline chunk of frames at a time (results are per frame), then the
+        # external-noise chain with the reference's op order
+        B = int(frames.shape[0])
+        sub = B if B == 0 else pipeline_chunk(B, frames[0].numel() * frames.element_size())
+        if sub >= B:
+            noise = ops.grain_noise_torch_global(frames, tg["seed"], tg["philox_offset"], first_frame, tg["clip_frames"], tg["draw_frames"])
+            return self._apply(frames, first_frame, worker, noise, out, False)
+        out = torch.empty_like(frames) if out is None else out
+        for i in range(0, B, sub):
+            f = frames[i:i + sub]
+            noise = ops.grain_noise_torch_global(f, tg["seed"], tg["philox_offset"], first_frame + i, tg["clip_frames"], tg["draw_frames"])
+            self._apply(f, first_frame + i, worker, noise, out[i:i + sub], False)
+            del noise
+        return out
+
+    def _apply(self, frames, first_frame, worker, ext_noise, out, fast_math):
+        """_run on the chain's own noise source or on ext_noise"""
         keep = []
         if self.colormatch is not None and not self.split and self.timing is None:
             d = self._desc(frames, first_frame, keep, ext_noise, fused_cm=True)
@@ -196,6 +232,7 @@ class PostChain:
         device, each streamed by its own host thread into its slice of one result (stream_frames_sharded); the result is
         bit-identical to one device's."""
         self.check_frames(frames_cpu)
+        self._torch_global(frames_cpu, None)
         if len(self.devices) == 1:
             return stream_frames(frames_cpu, lambda f, i: self(f, first_frame + i), chunk_frames, torch.device("cpu"), self.device, out=out)
         return stream_frames_sharded(frames_cpu, self.make_fn(first_frame), chunk_frames, torch.device("cpu"), self.devices, out=out)

@@ -10,9 +10,9 @@
 import torch
 
 from . import _native as nv
-from ._runtime import compute_device, devices_from_env, result_device, run_frames, upload
+from ._runtime import compute_device, devices_from_env, grain_noise_from_env, result_device, run_frames, upload
 from .chain import PostChain
-from .filter_nodes import _as_frames, draw_seed
+from .filter_nodes import GlobalStreamDraws, _as_frames, draw_seed
 from .lut_nodes import NO_LUTS, VRGDG_LUTS, _list_lut_files
 from .video_enhance import restore_frames
 
@@ -30,7 +30,9 @@ class VRGDG_B200_PostChain:
     """grain -> [colour match] -> 3D LUT -> sharpen in one pass over HBM (chain.PostChain).  Stage semantics and widget ranges
     are those of the four reference nodes (nodes.py:20-34, :72-84, :135-147; VRGDG_IV_Adjustments.py:145-157).  RGBA batches take
     the LUT and the sharpeners the reference runs on 4 channels: grain_intensity 0, no reference_image, and use_gpu=False for
-    laplacian / sobel."""
+    laplacian / sobel.  With VRGDG_GRAIN_NOISE=torch_cuda (read at call time) the grain is FastFilmGrain(images, grain_intensity,
+    saturation_mix, batch_size)'s in that mode, drawn from the compute device's global CUDA generator, which is advanced as that
+    node advances it."""
 
     @classmethod
     def INPUT_TYPES(cls):
@@ -45,7 +47,7 @@ class VRGDG_B200_PostChain:
                 "sharpen": (list(_SHARPENERS), {"default": "unsharp"}),
                 "sharpen_strength": ("FLOAT", {"default": 0.5, "min": 0.0, "max": 10.0, "step": 0.01}),
                 "use_gpu": ("BOOLEAN", {"default": False, "tooltip": "False: the reference's NumPy-path semantics (edge-replicated border); True: its torch path (zero padding)"}),
-                "batch_size": ("INT", {"default": 8, "min": 0, "max": 500, "step": 1, "tooltip": "frames per upload chunk (device memory bound); results do not depend on it"}),
+                "batch_size": ("INT", {"default": 8, "min": 0, "max": 500, "step": 1, "tooltip": "frames per upload chunk (device memory bound); results do not depend on it, except with VRGDG_GRAIN_NOISE=torch_cuda, where it is also the grain's draw size (0 = the whole batch), as FastFilmGrain's batch_size is"}),
             },
             "optional": {"reference_image": ("IMAGE",)},
         }
@@ -68,8 +70,13 @@ class VRGDG_B200_PostChain:
             if use_gpu and _SHARPENERS[sharpen][1] in (nv.STENCIL_LAPLACIAN_GPU, nv.STENCIL_SOBEL_GPU):
                 raise ValueError("VRGDG_B200_PostChain: sharpen=%s with use_gpu=True takes 3-channel images (the torch path convolves "
                                  "with groups=3), got 4 channels" % sharpen)
+        # the global stream's refusals come before any generator or device work
+        draws = GlobalStreamDraws(images, batch_size, "VRGDG_B200_PostChain") \
+            if float(grain_intensity) > 0 and grain_noise_from_env() == "torch_cuda" else None
         dev = compute_device(images)
-        grain = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), seed=draw_seed()) if float(grain_intensity) > 0 else None
+        grain = None
+        if draws is None and float(grain_intensity) > 0:
+            grain = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), seed=draw_seed())
         cm = None
         if reference_image is not None:
             ref = _as_frames(reference_image, "reference_image")
@@ -83,11 +90,16 @@ class VRGDG_B200_PostChain:
         op = _SHARPENERS[sharpen][1 if use_gpu else 0]
         if op != nv.STENCIL_NONE:
             stencil = dict(op=op, strength=float(sharpen_strength), border=nv.BORDER_ZERO if use_gpu else nv.BORDER_REPLICATE)
-        if grain is None and cm is None and lut is None and stencil is None:
+        if grain is None and draws is None and cm is None and lut is None and stencil is None:
             return (images,)
         devs = devices_from_env() if images.device.type == "cpu" else None
+        if draws is not None:
+            grain = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), torch_global=draws.snapshot(images)[1])
         chain = PostChain(grain=grain, colormatch=cm, lut=lut, stencil=stencil, device=None if devs else dev, devices=devs)
-        return (run_frames(images, chain.make_fn(), batch_size, result_device(images), chain.device, devs),)
+        out = run_frames(images, chain.make_fn(), batch_size, result_device(images), chain.device, devs)
+        if draws is not None:
+            draws.advance()
+        return (out,)
 
 
 class VRGDG_B200_EnhanceFrames:

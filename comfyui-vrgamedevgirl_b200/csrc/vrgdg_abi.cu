@@ -312,12 +312,17 @@ int vrgdg_grain(const void* in, void* out, int B, int H, int W, int dtype, float
   return VRGDG_OK;
 }
 
-int vrgdg_grain_torch_global(const void* in, void* out, int B, int H, int W, int dtype, float intensity, float sat, float one_minus_sat,
-                             uint64_t seed, uint64_t philox_offset, int64_t frame0, int64_t clip_frames, int64_t draw_frames,
-                             void* stream) {
-  const char* who = "vrgdg_grain_torch_global";
-  int rc = check_frames(in, out, B, H, W, dtype, who);
-  if (rc) return rc;
+}  // extern "C"
+
+namespace {
+
+// The global generator's draw geometry of frames [frame0, frame0 + B) (vrgdg_grain_torch_global, vrgdg_grain_noise_torch_global):
+// every refusal before any CUDA call, then, for a non-empty batch, the launch context and the 32-bit geometry on the current device.
+// `empty` = nothing to draw (VRGDG_OK without a CUDA call).
+struct TorchGlobalGeom { uint32_t step, clip, n, T_full, T_last; };
+int torch_global_prepare(int B, int H, int W, int dtype, uint64_t philox_offset, int64_t frame0, int64_t clip_frames, int64_t draw_frames,
+                         void* stream, const char* who, bool& empty, LaunchCtx& ctx, TorchGlobalGeom& g) {
+  empty = true;
   if (dtype == VRGDG_U8BGR) return fail(VRGDG_E_UNSUPPORTED, "%s: takes float frames (IMAGE tensors); uint8 frames are not drawn this way", who);
   if (philox_offset % 4) return fail(VRGDG_E_INVALID, "%s: Philox offset %llu is not a multiple of 4", who, (unsigned long long)philox_offset);
   if (draw_frames < 1) return fail(VRGDG_E_INVALID, "%s: draw_frames %lld < 1", who, (long long)draw_frames);
@@ -327,21 +332,63 @@ int vrgdg_grain_torch_global(const void* in, void* out, int B, int H, int W, int
   if ((int64_t)B * H * W == 0) return VRGDG_OK;
   const int64_t n = (int64_t)H * W * 3, step = draw_frames < clip_frames ? draw_frames : clip_frames;
   // every draw fits when the first (full) one does; checking one frame first keeps step * n from overflowing
+  int rc;
   if ((rc = check_torch_draw(n, torch_draw_es(dtype), who)) || (rc = check_torch_draw(step * n, torch_draw_es(dtype), who))) return rc;
-  LaunchCtx ctx;
   if ((rc = get_ctx(stream, ctx))) return rc;
+  empty = false;
+  // every index below is 32-bit now: clip_frames <= INT32_MAX and step * n <= INT32_MAX
+  g.step = (uint32_t)step; g.clip = (uint32_t)clip_frames; g.n = (uint32_t)n;
+  g.T_full = torch_randn_threads((uint64_t)(step * n), ctx.sms, ctx.threads_per_sm);
+  const uint32_t last = torch_global_draw(g.clip - 1, g.step);
+  g.T_last = torch_randn_threads(torch_global_numel(last, g.step, g.clip, g.n), ctx.sms, ctx.threads_per_sm);
+  return VRGDG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vrgdg_grain_torch_global(const void* in, void* out, int B, int H, int W, int dtype, float intensity, float sat, float one_minus_sat,
+                             uint64_t seed, uint64_t philox_offset, int64_t frame0, int64_t clip_frames, int64_t draw_frames,
+                             void* stream) {
+  const char* who = "vrgdg_grain_torch_global";
+  int rc = check_frames(in, out, B, H, W, dtype, who);
+  if (rc) return rc;
+  bool empty;
+  LaunchCtx ctx;
+  TorchGlobalGeom g;
+  if ((rc = torch_global_prepare(B, H, W, dtype, philox_offset, frame0, clip_frames, draw_frames, stream, who, empty, ctx, g)) || empty)
+    return rc;
   PointParams P;
   zero_point(P, B, H, W);
   P.gI = intensity; P.gs = sat; P.goms = one_minus_sat;
   P.seed = seed; P.frame0 = frame0; P.seed_mode = SEED_TORCH_GLOBAL;
-  // every index below is 32-bit now: clip_frames <= INT32_MAX and step * n <= INT32_MAX
-  P.toffset = philox_offset; P.tstep = (uint32_t)step; P.tclip = (uint32_t)clip_frames;
-  P.tT = torch_randn_threads((uint64_t)(step * n), ctx.sms, ctx.threads_per_sm);
-  const uint32_t last = torch_global_draw(P.tclip - 1, P.tstep);
-  P.tT_last = torch_randn_threads(torch_global_numel(last, P.tstep, P.tclip, (uint32_t)n), ctx.sms, ctx.threads_per_sm);
+  P.toffset = philox_offset; P.tstep = g.step; P.tclip = g.clip; P.tT = g.T_full; P.tT_last = g.T_last;
 #define PT(T) launch_point<T>(in, out, P, ST_GRAIN, true, ctx)
   cudaError_t e = DISPATCH_DTYPE(dtype, PT);
 #undef PT
+  if (e != cudaSuccess) return fail_cuda(e, who);
+  return VRGDG_OK;
+}
+
+int vrgdg_grain_noise_torch_global(void* noise, int B, int H, int W, int dtype, uint64_t seed, uint64_t philox_offset, int64_t frame0,
+                                   int64_t clip_frames, int64_t draw_frames, void* stream) {
+  const char* who = "vrgdg_grain_noise_torch_global";
+  int rc = check_frames(noise, noise, B, H, W, dtype, who);
+  if (rc) return rc;
+  bool empty;
+  LaunchCtx ctx;
+  TorchGlobalGeom g;
+  if ((rc = torch_global_prepare(B, H, W, dtype, philox_offset, frame0, clip_frames, draw_frames, stream, who, empty, ctx, g)) || empty)
+    return rc;
+  // rows x blocks per row is about the window's elements / 1024: beyond 2^31 only for windows no device holds
+  if (torch_global_window_rows((uint32_t)frame0, (uint32_t)B, g.n, g.step, g.T_full) * (g.T_full / TORCH_RANDN_BLOCK) >= ((uint64_t)1 << 31))
+    return fail(VRGDG_E_UNSUPPORTED, "%s: a window of %d frames has too many work items for one launch; split the batch", who, B);
+  const TorchGlobalWindow w = torch_global_window((uint32_t)frame0, (uint32_t)B, g.n, g.step, g.clip, g.T_full, g.T_last);
+  cudaError_t e;
+  if (dtype == VRGDG_F32) e = launch_torch_global_noise<float>(noise, seed, philox_offset, w, ctx);
+  else if (dtype == VRGDG_F16) e = launch_torch_global_noise<__half>(noise, seed, philox_offset, w, ctx);
+  else e = launch_torch_global_noise<__nv_bfloat16>(noise, seed, philox_offset, w, ctx);
   if (e != cudaSuccess) return fail_cuda(e, who);
   return VRGDG_OK;
 }

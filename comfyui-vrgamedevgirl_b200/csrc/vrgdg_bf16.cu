@@ -3,4 +3,5 @@
 namespace vrgdg {
 VRGDG_INSTANTIATE(__nv_bfloat16)
 VRGDG_INSTANTIATE_CODECS(__nv_bfloat16)
+VRGDG_INSTANTIATE_FLOAT(__nv_bfloat16)
 }

@@ -3,4 +3,5 @@
 namespace vrgdg {
 VRGDG_INSTANTIATE(__half)
 VRGDG_INSTANTIATE_CODECS(__half)
+VRGDG_INSTANTIATE_FLOAT(__half)
 }

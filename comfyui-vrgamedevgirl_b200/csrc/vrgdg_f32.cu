@@ -3,4 +3,5 @@
 namespace vrgdg {
 VRGDG_INSTANTIATE(float)
 VRGDG_INSTANTIATE_CODECS(float)
+VRGDG_INSTANTIATE_FLOAT(float)
 }

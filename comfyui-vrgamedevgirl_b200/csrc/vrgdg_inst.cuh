@@ -218,6 +218,20 @@ cudaError_t launch_moments(const void* in, const PointParams& P, bool grain, int
   return cudaGetLastError();
 }
 
+// ---- the global generator's noise, materialised --------------------------------------------------------
+// float dtypes only (the ABI refuses uint8 frames first); w.rows * T_full / 256 < 2^31 is the ABI's check
+template <typename T>
+cudaError_t launch_torch_global_noise(void* out, uint64_t seed, uint64_t o0, const TorchGlobalWindow& w, const LaunchCtx& ctx) {
+  const uint32_t blocks_full = w.T_full / TORCH_RANDN_BLOCK, total = w.rows * blocks_full;
+  if (total == 0) return cudaSuccess;
+  auto kern = k_torch_global_noise<T>;
+  static int occ = occupancy_of(kern, 256, 0);
+  const int grid = (int)std::min<int64_t>(total, (int64_t)ctx.sms * occ);
+  kern<<<grid, 256, 0, ctx.stream>>>(reinterpret_cast<T*>(out), seed, o0, w, blocks_full);
+  count_launch();
+  return cudaGetLastError();
+}
+
 // ---- u8 codecs ---------------------------------------------------------------------------------
 template <typename T>
 cudaError_t launch_u8_in(const uint8_t* in, void* out, int64_t npix, const LaunchCtx& ctx) {
@@ -255,5 +269,9 @@ cudaError_t launch_u8_out(const void* in, uint8_t* out, int64_t npix, const Laun
 #define VRGDG_INSTANTIATE_CODECS(T)                                                                                       \
   template cudaError_t launch_u8_in<T>(const uint8_t*, void*, int64_t, const LaunchCtx&);                                 \
   template cudaError_t launch_u8_out<T>(const void*, uint8_t*, int64_t, const LaunchCtx&);
+
+// float frame dtypes only: launchers with no uint8 counterpart
+#define VRGDG_INSTANTIATE_FLOAT(T)                                                                                        \
+  template cudaError_t launch_torch_global_noise<T>(void*, uint64_t, uint64_t, const TorchGlobalWindow&, const LaunchCtx&);
 
 }  // namespace vrgdg

@@ -310,6 +310,32 @@ k_grain_noise(float* __restrict__ out, int B, int W, int64_t hw, uint64_t seed, 
   }
 }
 
+// The global generator's N(0,1) values of a window of frames, in the frame dtype (torch_global_window): a block-stride loop over
+// (row, 256-thread block of the row), blocks_full = T_full / 256 blocks per row.  One Philox call and two Box-Muller evaluations per
+// work item (the sin / cos lanes of each pair share their log, sqrt and sincos), each value z * 1 + 0 in fp32 cast to T as ATen casts
+// it.  Stores of consecutive threads are consecutive elements.
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_torch_global_noise(T* __restrict__ out, uint64_t seed, uint64_t o0, TorchGlobalWindow w, uint32_t blocks_full) {
+  const uint32_t total = w.rows * blocks_full;
+  for (uint32_t rb = blockIdx.x; rb < total; rb += gridDim.x) {
+    const uint32_t r = rb / blocks_full, idx = (rb - r * blocks_full) * 256u + threadIdx.x;
+    TorchGlobalItem it;
+    if (!torch_global_item(w, r, idx, it)) continue;
+    TorchSite s;
+    s.k = it.k; s.ii = 0; s.idx = idx;
+    const U4 b = torch_randn_bits(seed, s, torch_global_offset(o0, it.j, w.step, w.n, w.T_full) >> 2);
+    float z[4];
+    z[0] = torch_box_muller(b.x, b.y, false); z[1] = torch_box_muller(b.x, b.y, true);
+    z[2] = torch_box_muller(b.z, b.w, false); z[3] = torch_box_muller(b.z, b.w, true);
+#pragma unroll
+    for (uint32_t ii = 0; ii < 4; ++ii) {
+      const uint32_t li = torch_global_li(it, idx, ii);
+      if (li >= it.lo && li < it.hi) out[it.base + li] = Elem<T>::st(z[ii]);
+    }
+  }
+}
+
 // =====================================================================================================
 // mbarrier / TMA primitives (inline PTX; SASS: SYNCS.*, UTMALDG)
 // =====================================================================================================
@@ -1219,6 +1245,8 @@ template <typename T> cudaError_t launch_tile_rgba_lut(const CUtensorMap* tmap, 
 template <typename T> cudaError_t launch_moments(const void* in, const PointParams& P, bool grain, int row0, int rows,
                                                  double* sums, double* partials, const LaunchCtx& ctx, float* fplanes = nullptr,
                                                  bool small_blocks = false);
+template <typename T> cudaError_t launch_torch_global_noise(void* out, uint64_t seed, uint64_t o0, const TorchGlobalWindow& w,
+                                                            const LaunchCtx& ctx);
 template <typename T> cudaError_t launch_u8_in(const uint8_t* in, void* out, int64_t npix, const LaunchCtx& ctx);
 template <typename T> cudaError_t launch_u8_out(const void* in, uint8_t* out, int64_t npix, const LaunchCtx& ctx);
 template <typename T> void tile_geometry(int H, int RW, int& tiles_x, int& tiles_y, int& box_x, int& box_y);

@@ -327,6 +327,81 @@ VRGDG_HD uint64_t torch_global_offset(uint64_t o0, uint32_t j, uint32_t step, ui
   return o0 + (uint64_t)j * torch_randn_increment<uint32_t>(step * n, T_full);
 }
 
+// ---- the global stream materialised (k_torch_global_noise, vrgdg_grain_noise_torch_global) ---------------------------------
+// The N(0,1) values of frames [frame0, frame0 + frames) of the clip, written with ATen's own thread -> element mapping: a work item
+// (draw j, iteration k, thread idx < T_j) makes one Philox call and stores its four normals to elements li = 4 T_j k + T_j ii + idx
+// (ii = 0..3) of draw j that lie in the window.  Rows (j, k) are numbered over the draws the window touches: the first draw's rows
+// from its window's first iteration, then every row of the full draws in between, then the last draw's rows up to its window's end.
+struct TorchGlobalWindow {
+  uint32_t frame0, frames, n, step, clip, T_full, T_last;
+  uint32_t j0, j1;             // first and last draw the window touches
+  uint32_t ka0, rows0;         // draw j0: first iteration in the window, rows
+  uint32_t k_mid, rows_mid;    // draws j0 < j < j1 (full, whole): rows of each, rows of all
+  uint32_t ka1, rows1;         // draw j1 when j1 > j0 (rows1 = 0 otherwise)
+  uint32_t rows;
+};
+
+// draw-local elements [lo, hi) of draw j that the window holds
+VRGDG_HD void torch_global_draw_window(const TorchGlobalWindow& w, uint32_t j, uint32_t& lo, uint32_t& hi) {
+  const uint32_t first = j * w.step, end = w.frame0 + w.frames, dend = first + w.step;
+  lo = ((w.frame0 > first ? w.frame0 : first) - first) * w.n;
+  hi = ((end < dend ? end : dend) - first) * w.n;
+}
+
+// frames >= 1, n >= 1, frame0 + frames <= clip; the caller keeps the row count below 2^32 (it is about elements / 4T)
+VRGDG_HD TorchGlobalWindow torch_global_window(uint32_t frame0, uint32_t frames, uint32_t n, uint32_t step, uint32_t clip,
+                                               uint32_t T_full, uint32_t T_last) {
+  TorchGlobalWindow w;
+  w.frame0 = frame0; w.frames = frames; w.n = n; w.step = step; w.clip = clip; w.T_full = T_full; w.T_last = T_last;
+  w.j0 = torch_global_draw(frame0, step);
+  w.j1 = torch_global_draw(frame0 + frames - 1, step);
+  uint32_t lo, hi, T4;
+  torch_global_draw_window(w, w.j0, lo, hi);
+  T4 = 4u * torch_global_threads(w.j0, step, clip, T_full, T_last);
+  w.ka0 = lo / T4;
+  w.rows0 = (hi - 1) / T4 - w.ka0 + 1;
+  w.k_mid = (step * n - 1) / (4u * T_full) + 1;
+  w.rows_mid = w.j1 > w.j0 ? (w.j1 - w.j0 - 1) * w.k_mid : 0u;
+  w.ka1 = w.rows1 = 0;
+  if (w.j1 > w.j0) {
+    torch_global_draw_window(w, w.j1, lo, hi);
+    T4 = 4u * torch_global_threads(w.j1, step, clip, T_full, T_last);
+    w.ka1 = lo / T4;
+    w.rows1 = (hi - 1) / T4 - w.ka1 + 1;
+  }
+  w.rows = w.rows0 + w.rows_mid + w.rows1;
+  return w;
+}
+
+// row count of a window in 64 bits, for the caller's check that it fits the 32-bit rows above
+VRGDG_HD uint64_t torch_global_window_rows(uint32_t frame0, uint32_t frames, uint32_t n, uint32_t step, uint32_t T_full) {
+  const uint64_t draws = (uint64_t)torch_global_draw(frame0 + frames - 1, step) - torch_global_draw(frame0, step) + 1;
+  return draws * ((uint64_t)(step * n - 1) / (4u * (uint64_t)T_full) + 1);
+}
+
+// work item (row r < w.rows, thread idx) -> draw j, iteration k, T_j, the draw's window [lo, hi), and the index of draw element 0 in
+// the window's [frames, H, W, 3] tensor (negative when the draw starts before the window).  False when idx >= T_j (a row of the
+// clip's last draw, launched T_full threads wide).
+struct TorchGlobalItem { uint32_t j, k, T, lo, hi; int64_t base; };
+VRGDG_HD bool torch_global_item(const TorchGlobalWindow& w, uint32_t r, uint32_t idx, TorchGlobalItem& it) {
+  if (r < w.rows0) {
+    it.j = w.j0; it.k = w.ka0 + r;
+  } else if (r - w.rows0 < w.rows_mid) {
+    const uint32_t m = r - w.rows0, q = m / w.k_mid;
+    it.j = w.j0 + 1u + q; it.k = m - q * w.k_mid;
+  } else {
+    it.j = w.j1; it.k = w.ka1 + (r - w.rows0 - w.rows_mid);
+  }
+  it.T = torch_global_threads(it.j, w.step, w.clip, w.T_full, w.T_last);
+  if (idx >= it.T) return false;
+  torch_global_draw_window(w, it.j, it.lo, it.hi);
+  it.base = ((int64_t)it.j * w.step - (int64_t)w.frame0) * (int64_t)w.n;
+  return true;
+}
+
+// element of lane ii of a work item (ATen: linear_index + T * ii, linear_index = 4 T k + idx)
+VRGDG_HD uint32_t torch_global_li(const TorchGlobalItem& it, uint32_t idx, uint32_t ii) { return 4u * it.T * it.k + it.T * ii + idx; }
+
 // the reference's grain mix of channel c (RGB) alone, one rounding per op: s * z'_c + (1 - s) * z_g, z' = (2 z_r, z_g, 3 z_b)
 VRGDG_HD float grain_mix_exact(float zc, float zg, int c, float s, float oms) {
   const float zs = (c == 0) ? mulx(zc, 2.0f) : ((c == 2) ? mulx(zc, 3.0f) : zc);

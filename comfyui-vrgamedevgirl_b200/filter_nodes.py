@@ -63,31 +63,51 @@ class FastFilmGrain:
         return (out,)
 
 
+class GlobalStreamDraws:
+    """The generator bookkeeping of grain drawn as FastFilmGrain draws it under VRGDG_GRAIN_NOISE=torch_cuda (nodes.py:46-62 on a CUDA
+    device): torch.randn_like once per mini-batch of batch_size frames (0 = the whole batch) from the compute device's global CUDA
+    generator, which those draws leave advanced.  The constructor only checks the draws (a draw past 32-bit indexing raises
+    ValueError) and touches neither a generator nor a device; snapshot() reads the generator, advance() moves it past the draws
+    afterwards.  The CPU generator is never touched (the reference does not touch it either)."""
+
+    def __init__(self, images, batch_size, who):
+        B, H, W = (int(s) for s in images.shape[:3])
+        self.B, self.n = B, H * W * 3
+        self.step = min(int(batch_size), B) if int(batch_size) > 0 else B      # nodes.py:46; one draw when batch_size >= B
+        if B > 0 and self.n > 0 and 1 + (self.step * self.n - 1) * images.element_size() > 2**31 - 1:
+            raise ValueError("vrgdg_b200: %s with VRGDG_GRAIN_NOISE=torch_cuda: a draw of %d frames of %dx%d (batch_size=%d) exceeds "
+                             "32-bit indexing (torch splits such a draw into sub-draws, which is not reproduced); lower batch_size"
+                             % (who, self.step, W, H, int(batch_size)))
+        self._gen = None
+
+    def snapshot(self, images):
+        """(device, dict(seed, philox_offset, clip_frames, draw_frames)): the compute device's generator as the draws find it"""
+        dev = cuda_device(compute_device(images))
+        torch.cuda.init()
+        self._gen = torch.cuda.default_generators[dev.index]
+        self._offset = self._gen.get_offset()
+        self._total = 0
+        if self.B > 0 and self.n > 0:
+            self._total = (self.B // self.step) * ops.torch_randn_increment(self.step * self.n, dev) + \
+                ops.torch_randn_increment((self.B % self.step) * self.n, dev)
+        return dev, dict(seed=self._gen.initial_seed(), philox_offset=self._offset, clip_frames=self.B, draw_frames=self.step)
+
+    def advance(self):
+        """the generator's offset after the draws, as the reference's draws leave it"""
+        self._gen.set_offset(self._offset + self._total)
+
+
 def _global_stream_grain(images, intensity, sat, batch_size):
-    """FastFilmGrain with VRGDG_GRAIN_NOISE=torch_cuda: the noise the reference draws on a CUDA device, torch.randn_like once per
-    mini-batch of batch_size frames (0 = the whole batch) from the compute device's global generator, and that generator advanced
-    as those draws advance it.  Unlike the default path, the grain here depends on batch_size, as the reference's does.  The
-    CPU generator is not touched (the reference does not touch it either)."""
-    B, H, W = (int(s) for s in images.shape[:3])
-    step = min(int(batch_size), B) if int(batch_size) > 0 else B            # nodes.py:46; one draw when batch_size >= B
-    n = H * W * 3
-    if B > 0 and n > 0 and 1 + (step * n - 1) * images.element_size() > 2**31 - 1:
-        raise ValueError("vrgdg_b200: FastFilmGrain with VRGDG_GRAIN_NOISE=torch_cuda: a draw of %d frames of %dx%d (batch_size=%d) "
-                         "exceeds 32-bit indexing (torch splits such a draw into sub-draws, which is not reproduced); lower batch_size"
-                         % (step, W, H, int(batch_size)))
-    dev = cuda_device(compute_device(images))
-    torch.cuda.init()
-    gen = torch.cuda.default_generators[dev.index]
-    seed, offset = gen.initial_seed(), gen.get_offset()
-    total = 0
-    if B > 0 and n > 0:
-        total = (B // step) * ops.torch_randn_increment(step * n, dev) + ops.torch_randn_increment((B % step) * n, dev)
+    """FastFilmGrain with VRGDG_GRAIN_NOISE=torch_cuda: the noise the reference draws on a CUDA device (GlobalStreamDraws).  Unlike
+    the default path, the grain here depends on batch_size, as the reference's does."""
+    draws = GlobalStreamDraws(images, batch_size, "FastFilmGrain")
+    dev, g = draws.snapshot(images)
 
     def run(frames, first):
-        return ops.grain_torch_global(frames, intensity, sat, 1.0 - sat, seed, offset, first, B, step)
+        return ops.grain_torch_global(frames, intensity, sat, 1.0 - sat, g["seed"], g["philox_offset"], first, g["clip_frames"], g["draw_frames"])
     devs = devices_from_env() if images.device.type == "cpu" else None
     out = run_frames(images, lambda card: run, batch_size, result_device(images), dev, devs)
-    gen.set_offset(offset + total)
+    draws.advance()
     return out
 
 

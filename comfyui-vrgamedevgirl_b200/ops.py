@@ -107,6 +107,21 @@ def grain_torch_global(images, intensity, sat, one_minus_sat, seed, philox_offse
     return out
 
 
+def grain_noise_torch_global(frames, seed, philox_offset, frame0, clip_frames, draw_frames):
+    """The N(0,1) tensor grain_torch_global draws for `frames` (frames [frame0, frame0 + B) of the clip), shaped like `frames` and in
+    their dtype: frame f's slice of the reference's torch.randn_like draw (vrgdg_grain_noise_torch_global).  It feeds the chain's
+    ext_noise.  The generator is not advanced here."""
+    t = _frames(frames)
+    out = torch.empty_like(t)
+    B, H, W, _ = t.shape
+    lib = nv.load_library()
+    with torch.cuda.device(t.device):
+        nv.check(lib.vrgdg_grain_noise_torch_global(nv.ptr(out), B, H, W, nv.DTYPE_CODE[t.dtype], ctypes.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF),
+                                                    ctypes.c_uint64(int(philox_offset) & 0xFFFFFFFFFFFFFFFF), ctypes.c_int64(int(frame0)),
+                                                    ctypes.c_int64(int(clip_frames)), ctypes.c_int64(int(draw_frames)), nv.stream_ptr(t.device)))
+    return out
+
+
 def torch_randn_increment(numel, device):
     """The Philox offset torch.randn of `numel` elements consumes on `device`'s CUDA generator (vrgdg_torch_randn_increment)."""
     inc = ctypes.c_int64(0)

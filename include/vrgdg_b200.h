@@ -161,6 +161,17 @@ VRGDG_API int vrgdg_grain_torch_global(const void* in, void* out, int B, int H, 
                              uint64_t seed, uint64_t philox_offset, int64_t frame0, int64_t clip_frames, int64_t draw_frames,
                              void* stream);
 
+/* The N(0,1) values vrgdg_grain_torch_global draws for frames [frame0, frame0 + B) of the clip, written to `noise`
+ * ([B,H,W,3] in the frame dtype, contiguous, RGB order): element (b, y, x, c) = element (f mod step) n + (y W + x) 3 + c of draw
+ * f / step, f = frame0 + b, in the stream described above, z * 1 + 0 in fp32 cast to the frame dtype (round to nearest) as
+ * torch.randn_like casts it.  So noise[b] equals frame f's slice of the reference's torch.randn_like draw, and a chain run with
+ * this tensor as ext_noise (vrgdg_chain_apply_ext, vrgdg_chain_cm_apply, vrgdg_chain_lab_moments_ext, exact arithmetic) grains
+ * the frames as FastFilmGrain does.  Written with ATen's thread -> element mapping: one Philox call per four normals, stores of
+ * consecutive threads to consecutive elements.  Same arguments, refusals (before any CUDA call) and SM rule as
+ * vrgdg_grain_torch_global; B == 0 or an empty frame is VRGDG_OK.  The generator is neither read nor advanced. */
+VRGDG_API int vrgdg_grain_noise_torch_global(void* noise, int B, int H, int W, int dtype, uint64_t seed, uint64_t philox_offset,
+                                   int64_t frame0, int64_t clip_frames, int64_t draw_frames, void* stream);
+
 /* *inc = the Philox offset torch.randn of numel elements consumes on the current device's CUDA generator: inc(numel) above
  * (0 for numel 0, without a CUDA call). */
 VRGDG_API int vrgdg_torch_randn_increment(int64_t numel, int64_t* inc);
