@@ -121,6 +121,7 @@ SIGNATURES = {
     "vrgdg_chain_lab_moments_ext": (_i, [_vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp, _vp, _vp, _i64, _vp]),
     "vrgdg_chain_cm_scratch_bytes": (_i64, [_i, _i, _i, _i, _i, _i]),
     "vrgdg_chain_cm_apply": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp, _i, _vp, _i, _vp, _i64, _i, _vp]),
+    "vrgdg_chain_cm_apply_refs": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.POINTER(ChainDesc), _vp, _i, _i, _vp, _vp, _i, _vp, _i64, _i, _vp]),
     "vrgdg_adjust_scratch_bytes": (_i64, [_i, _i, _i, ctypes.POINTER(AdjustDesc)]),
     "vrgdg_adjust": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.POINTER(AdjustDesc), _vp, _vp, _vp, _i64, _vp]),
     "vrgdg_resize": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ResizeDesc), _vp]),

@@ -24,7 +24,12 @@ class PostChain:
                             generator (filter_nodes.GlobalStreamDraws), so that the grain is FastFilmGrain's under
                             VRGDG_GRAIN_NOISE=torch_cuda: one randn_like per draw_frames frames of a clip of clip_frames frames.
                             The chain neither reads nor advances a generator; the frames' first_frame keys the draws.
-        colormatch:         dict(reference_image=[1,H,W,3] tensor  |  ref_sums=[1,7] float64, strength)
+        colormatch:         dict(reference_image=[1,H,W,3] tensor  |  reference_frames=[N,Hr,Wr,3] tensor  |  ref_sums=[1|N,7] float64,
+                            strength).  reference_frames / ref_sums with N > 1 are a reference CLIP: frame f of the clip (absolute
+                            index, first_frame + i) is matched to reference frame f, at every chunk size (ColorMatchToReference's
+                            pairing); a call whose frames reach past frame N - 1 raises ValueError before any device work.  Each
+                            call uploads only the reference frames of its own indices (host or CUDA, any size and float dtype; they
+                            are converted to the frames' dtype on the frames' card).  One reference frame is broadcast.
         lut:                dict(lut_data={"lut","domain_min","domain_max"}, strength 0..10)
         stencil:            dict(op=STENCIL_*, strength, border=BORDER_REPLICATE)
         devices:            CUDA devices run_host shards host batches over (default None: `device` alone).  The first one is `device`;
@@ -44,6 +49,7 @@ class PostChain:
         # per device: the packed LUT and the reference statistics (made on `device`, copied to the others); per (device, worker on
         # that device): the colour-match scratch
         self._luts, self._refs, self._scratch = {}, {}, {}
+        self._ref_frames = None     # the reference clip (reference_frames with more than one frame), where the caller keeps it
         self.timing = None          # set to a list to collect (moments_start, moments_end, apply_start, apply_end) CUDA events per call
         # colour-match schedule (vrgdg_chain_cm_apply): one library call; `split` = the three-call path (statistics, parameters,
         # apply as separate entry points; what `timing` needs), `recompute` / `group_frames`: see include/vrgdg_b200.h
@@ -53,7 +59,16 @@ class PostChain:
             self._luts = {dev: packed if dev == self.device else ops.PackedLut(packed.data.to(dev), packed.size)
                           for dev in dict.fromkeys(self.devices)}
         if colormatch is not None:
-            self.set_reference(colormatch.get("reference_image"), colormatch.get("ref_sums"))
+            frames = colormatch.get("reference_frames")
+            if frames is not None:
+                if not isinstance(frames, torch.Tensor) or frames.ndim != 4 or frames.shape[-1] != 3 or frames.shape[0] < 1:
+                    raise ValueError("vrgdg_b200: PostChain colormatch reference_frames must be a tensor [N,H,W,3] with N >= 1")
+                if colormatch.get("reference_image") is not None or colormatch.get("ref_sums") is not None:
+                    raise ValueError("vrgdg_b200: PostChain colormatch takes one of reference_image, reference_frames, ref_sums")
+            if frames is not None and frames.shape[0] > 1:
+                self._ref_frames = frames
+            else:
+                self.set_reference(colormatch.get("reference_image") if frames is None else frames, colormatch.get("ref_sums"))
 
     # -- colour-match reference statistics (the only cross-rank quantity, see dist.py) --
     def set_reference(self, reference_image=None, ref_sums=None):
@@ -66,6 +81,30 @@ class PostChain:
         else:
             raise ValueError("colour match needs reference_image or ref_sums")
         self._refs = {dev: sums if dev == self.device else sums.to(dev) for dev in dict.fromkeys(self.devices)}
+        self._ref_frames = None
+
+    def _n_ref(self):
+        """frames in the reference: 1 (broadcast) or the length of a reference clip; None without colour match"""
+        if self.colormatch is None:
+            return None
+        return int(self._ref_frames.shape[0]) if self._ref_frames is not None else int(self._ref_sums.shape[0])
+
+    def check_reference(self, n_frames, first_frame):
+        """A reference clip pairs by absolute frame index: frames [first_frame, first_frame + n_frames) need as many reference frames.
+        ValueError otherwise, before any device work."""
+        n_ref = self._n_ref()
+        if n_ref is not None and n_ref != 1 and int(first_frame) + int(n_frames) > n_ref:
+            raise ValueError("vrgdg_b200: PostChain colour match has a reference clip of %d frames, but the frames are [%d, %d) of the clip"
+                             % (n_ref, int(first_frame), int(first_frame) + int(n_frames)))
+
+    def _reference_for(self, frames, first_frame):
+        """(reference frames, None) or (None, reference sums) for frames [first_frame, first_frame + B) on frames.device: the
+        reference clip's frames of those indices, uploaded and converted to the frames' dtype there, or the sums' rows"""
+        B = int(frames.shape[0])
+        if self._ref_frames is not None:
+            return upload(self._ref_frames[first_frame:first_frame + B], frames.device).to(frames.dtype), None
+        sums = self._on(self._refs, frames.device)
+        return None, (sums if sums.shape[0] == 1 else sums[first_frame:first_frame + B])
 
     @property
     def _ref_sums(self):
@@ -122,11 +161,15 @@ class PostChain:
         elif self.colormatch is not None:
             # per-frame LAB moments of the colour-match INPUT (= grain output when grain is enabled): a first pass
             # that recomputes the counter-based grain instead of materialising it
+            ref, ref_sums = self._reference_for(frames, first_frame)
+            if ref is not None:
+                ref_sums = ops.lab_moments(ref)
+                del ref
             if self.timing is not None:
                 self._ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
                 self._ev[0].record()
             sums = ops.chain_lab_moments(frames, d, ext_noise=ext_noise)
-            params = ops.colormatch_params(sums, self._on(self._refs, frames.device))
+            params = ops.colormatch_params(sums, ref_sums)
             if self.timing is not None:
                 self._ev[1].record()
             keep.append(params)
@@ -170,6 +213,7 @@ class PostChain:
     def _run(self, frames, first_frame, worker, ext_noise=None, out=None, fast_math=False):
         """__call__ with the colour-match scratch of `worker` (the index of a stream_frames_sharded worker on the frames' device)."""
         self.check_frames(frames)
+        self.check_reference(frames.shape[0], first_frame)
         tg = self._torch_global(frames, ext_noise)
         if tg is None:
             return self._apply(frames, first_frame, worker, ext_noise, out, fast_math)
@@ -194,7 +238,13 @@ class PostChain:
         if self.colormatch is not None and not self.split and self.timing is None:
             d = self._desc(frames, first_frame, keep, ext_noise, fused_cm=True)
             key = (frames.device, worker)
-            res, self._scratch[key] = ops.chain_cm_apply(frames, d, self._on(self._refs, frames.device), ext_noise=ext_noise, out=out,
+            ref, ref_sums = self._reference_for(frames, first_frame)
+            if ref is not None:
+                res, self._scratch[key] = ops.chain_cm_apply_refs(frames, d, ref, ext_noise=ext_noise, out=out, fast_math=fast_math,
+                                                                  recompute=self.recompute, group_frames=self.group_frames,
+                                                                  scratch=self._scratch.get(key), serial=self.serial)
+                return res
+            res, self._scratch[key] = ops.chain_cm_apply(frames, d, ref_sums, ext_noise=ext_noise, out=out,
                                                          fast_math=fast_math, recompute=self.recompute, group_frames=self.group_frames,
                                                          scratch=self._scratch.get(key), serial=self.serial)
             return res
@@ -232,6 +282,7 @@ class PostChain:
         device, each streamed by its own host thread into its slice of one result (stream_frames_sharded); the result is
         bit-identical to one device's."""
         self.check_frames(frames_cpu)
+        self.check_reference(frames_cpu.shape[0], first_frame)
         self._torch_global(frames_cpu, None)
         if len(self.devices) == 1:
             return stream_frames(frames_cpu, lambda f, i: self(f, first_frame + i), chunk_frames, torch.device("cpu"), self.device, out=out)

@@ -30,7 +30,8 @@ class VRGDG_B200_PostChain:
     """grain -> [colour match] -> 3D LUT -> sharpen in one pass over HBM (chain.PostChain).  Stage semantics and widget ranges
     are those of the four reference nodes (nodes.py:20-34, :72-84, :135-147; VRGDG_IV_Adjustments.py:145-157).  RGBA batches take
     the LUT and the sharpeners the reference runs on 4 channels: grain_intensity 0, no reference_image, and use_gpu=False for
-    laplacian / sobel.  With VRGDG_GRAIN_NOISE=torch_cuda (read at call time) the grain is FastFilmGrain(images, grain_intensity,
+    laplacian / sobel.  reference_image holds one frame or one per frame, as ColorMatchToReference's does: with B frames, frame i is
+    matched to reference frame i at every batch_size, and each chunk uploads only its own reference frames.  With VRGDG_GRAIN_NOISE=torch_cuda (read at call time) the grain is FastFilmGrain(images, grain_intensity,
     saturation_mix, batch_size)'s in that mode, drawn from the compute device's global CUDA generator, which is advanced as that
     node advances it."""
 
@@ -70,6 +71,13 @@ class VRGDG_B200_PostChain:
             if use_gpu and _SHARPENERS[sharpen][1] in (nv.STENCIL_LAPLACIAN_GPU, nv.STENCIL_SOBEL_GPU):
                 raise ValueError("VRGDG_B200_PostChain: sharpen=%s with use_gpu=True takes 3-channel images (the torch path convolves "
                                  "with groups=3), got 4 channels" % sharpen)
+        ref = n_ref = None
+        if reference_image is not None:
+            # ColorMatchToReference's rule: one reference frame for every frame, or one per frame (frame i matched to reference i)
+            ref = _as_frames(reference_image, "reference_image")
+            n_ref = int(ref.shape[0])
+            if n_ref != 1 and n_ref != int(images.shape[0]):
+                raise ValueError("reference_image batch (%d) must be 1 or match images batch (%d)" % (n_ref, images.shape[0]))
         # the global stream's refusals come before any generator or device work
         draws = GlobalStreamDraws(images, batch_size, "VRGDG_B200_PostChain") \
             if float(grain_intensity) > 0 and grain_noise_from_env() == "torch_cuda" else None
@@ -79,10 +87,10 @@ class VRGDG_B200_PostChain:
             grain = dict(intensity=float(grain_intensity), saturation_mix=float(saturation_mix), seed=draw_seed())
         cm = None
         if reference_image is not None:
-            ref = _as_frames(reference_image, "reference_image")
-            if int(ref.shape[0]) != 1:
-                raise ValueError("VRGDG_B200_PostChain: reference_image must hold exactly one frame")
-            cm = dict(reference_image=ref.to(images.dtype), strength=float(match_strength))
+            if n_ref == 1:
+                cm = dict(reference_image=ref.to(images.dtype), strength=float(match_strength))
+            else:       # streamed: each chunk uploads the reference frames of its own indices
+                cm = dict(reference_frames=ref, strength=float(match_strength))
         lut = None
         if lut_name != _NONE and float(lut_strength) > 0:
             lut = dict(lut_data=VRGDG_LUTS._load_lut(lut_name), strength=float(lut_strength))

@@ -762,24 +762,34 @@ static int cm_streams(CmStreams*& out) {
   return VRGDG_OK;
 }
 
-int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc,
-                         const double* ref_sums, int n_ref, const void* ext_noise, int flags, void* scratch, int64_t scratch_bytes,
-                         int group_frames, void* stream) {
-  if (!desc) return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: null descriptor");
-  if (!desc->colormatch_enabled) return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: the descriptor has no colour-match stage (use vrgdg_chain_apply)");
-  int rc = check_frames(in, out, B, H, W, dtype, "vrgdg_chain_cm_apply");
+/* The reference frames of vrgdg_chain_cm_apply_refs: frame b of `frames` ([B][H][W][3], the frames' dtype) is frame b's reference;
+ * its sums go to sums[b] ([B][7] doubles), group by group, ahead of the parameters that read them. */
+struct CmRefFrames { const void* frames; int H, W; double* sums; };
+
+/* vrgdg_chain_cm_apply, or with `refs` vrgdg_chain_cm_apply_refs (then ref_sums == refs->sums and n_ref == B) */
+static int chain_cm_core(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc,
+                         const double* ref_sums, int n_ref, const CmRefFrames* refs, const void* ext_noise, int flags, void* scratch,
+                         int64_t scratch_bytes, int group_frames, void* stream, const char* who) {
+  if (!desc) return fail(VRGDG_E_INVALID, "%s: null descriptor", who);
+  if (!desc->colormatch_enabled) return fail(VRGDG_E_INVALID, "%s: the descriptor has no colour-match stage (use vrgdg_chain_apply)", who);
+  int rc = check_frames(in, out, B, H, W, dtype, who);
   if (rc) return rc;
-  if (n_ref != 1 && n_ref != B) return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: reference batch %d is neither 1 nor %d", n_ref, B);
-  if ((rc = check_chain_torch(desc, H, W, dtype, "vrgdg_chain_cm_apply"))) return rc;
+  if (n_ref != 1 && n_ref != B) return fail(VRGDG_E_INVALID, "%s: reference batch %d is neither 1 nor %d", who, n_ref, B);
+  if ((rc = check_chain_torch(desc, H, W, dtype, who))) return rc;
   if (desc->grain_enabled && desc->grain_seed_mode != VRGDG_SEED_PER_CLIP && desc->grain_seed_mode != VRGDG_SEED_PER_FRAME)
-    return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: bad grain seed_mode %d", desc->grain_seed_mode);
+    return fail(VRGDG_E_INVALID, "%s: bad grain seed_mode %d", who, desc->grain_seed_mode);
   if ((int64_t)B * H * W == 0) return VRGDG_OK;
-  if (!ref_sums || !scratch) return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: null pointer");
-  if (in == out) return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply cannot run in place");
-  if (reinterpret_cast<uintptr_t>(scratch) & 255u) return fail(VRGDG_E_ALIGN, "vrgdg_chain_cm_apply: scratch must be 256-byte aligned");
+  if (!ref_sums || !scratch) return fail(VRGDG_E_INVALID, "%s: null pointer", who);
+  if (in == out) return fail(VRGDG_E_INVALID, "%s cannot run in place", who);
+  if (reinterpret_cast<uintptr_t>(scratch) & 255u) return fail(VRGDG_E_ALIGN, "%s: scratch must be 256-byte aligned", who);
   if (scratch_bytes < vrgdg_chain_cm_scratch_bytes(B, H, W, dtype, flags, group_frames))
-    return fail(VRGDG_E_INVALID, "vrgdg_chain_cm_apply: scratch too small (%lld < %lld)", (long long)scratch_bytes,
+    return fail(VRGDG_E_INVALID, "%s: scratch too small (%lld < %lld)", who, (long long)scratch_bytes,
                 (long long)vrgdg_chain_cm_scratch_bytes(B, H, W, dtype, flags, group_frames));
+  if (refs) {
+    if (!refs->frames) return fail(VRGDG_E_INVALID, "%s: null ref_frames", who);
+    if (reinterpret_cast<uintptr_t>(refs->frames) % elem_size(dtype)) return fail(VRGDG_E_ALIGN, "%s: ref_frames not aligned to its element size", who);
+    if (reinterpret_cast<uintptr_t>(refs->sums) % 8) return fail(VRGDG_E_ALIGN, "%s: ref_sums must be 8-byte aligned", who);
+  }
   LaunchCtx ctx;
   if ((rc = get_ctx(stream, ctx))) return rc;
   const int G = cm_group_frames(B, H, W, dtype, flags, group_frames);
@@ -838,6 +848,17 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
     const void* gnoise = ext_noise ? reinterpret_cast<const char*>(ext_noise) + (size_t)g0 * H * W * 3 * noise_es : nullptr;
     const LaunchCtx& c1 = piped ? lo : ctx;
     cudaError_t e = cudaSuccess;
+    if (refs) {
+      // pass 0: the group's reference frames, vrgdg_lab_moments' instantiation (no grain, no f-planes) on the statistics stream, so in
+      // the pipelined schedule they run under the apply pass of the previous group too; partials[buf] is free, only this stream uses it
+      PointParams R;
+      zero_point(R, n, refs->H, refs->W);
+      const void* gref = reinterpret_cast<const char*>(refs->frames) + (size_t)g0 * refs->H * refs->W * 3 * es;
+#define RM(T) launch_moments<T>(gref, R, false, 0, refs->H, refs->sums + (int64_t)g0 * 7, partials[buf], c1)
+      e = DISPATCH_DTYPE(dtype, RM);
+#undef RM
+      if (e != cudaSuccess) { cleanup(); return fail_cuda(e, "vrgdg_chain_cm_apply_refs (reference moments)"); }
+    }
     if (piped && gi >= 2) e = cudaStreamWaitEvent(lo.stream, ev_p2[buf], 0);      // the apply pass of group gi-2 has released this buffer
     if (e != cudaSuccess) { cleanup(); return fail_cuda(e, "vrgdg_chain_cm_apply (wait)"); }
     // pass 1: grain (recomputed from the counter-based generator or read from ext_noise) -> Lab statistics [+ f-planes]
@@ -876,6 +897,24 @@ int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dty
     if (e != cudaSuccess) return fail_cuda(e, "vrgdg_chain_cm_apply (join)");
   }
   return VRGDG_OK;
+}
+
+int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc,
+                         const double* ref_sums, int n_ref, const void* ext_noise, int flags, void* scratch, int64_t scratch_bytes,
+                         int group_frames, void* stream) {
+  return chain_cm_core(in, out, B, H, W, dtype, desc, ref_sums, n_ref, nullptr, ext_noise, flags, scratch, scratch_bytes, group_frames,
+                       stream, "vrgdg_chain_cm_apply");
+}
+
+int vrgdg_chain_cm_apply_refs(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc,
+                              const void* ref_frames, int Hr, int Wr, double* ref_sums, const void* ext_noise, int flags, void* scratch,
+                              int64_t scratch_bytes, int group_frames, void* stream) {
+  const char* who = "vrgdg_chain_cm_apply_refs";
+  if (dtype == VRGDG_U8BGR) return fail(VRGDG_E_UNSUPPORTED, "%s: uint8 frames are not supported (reference clips are float IMAGE tensors)", who);
+  if (Hr < 1 || Wr < 1) return fail(VRGDG_E_INVALID, "%s: bad reference frame size %d x %d", who, Hr, Wr);
+  if ((int64_t)Hr * Wr >= (int64_t)1 << 31) return fail(VRGDG_E_UNSUPPORTED, "%s: reference frame of %d x %d pixels exceeds 2^31", who, Hr, Wr);
+  const CmRefFrames refs = {ref_frames, Hr, Wr, ref_sums};
+  return chain_cm_core(in, out, B, H, W, dtype, desc, ref_sums, B, &refs, ext_noise, flags, scratch, scratch_bytes, group_frames, stream, who);
 }
 
 int64_t vrgdg_adjust_scratch_bytes(int B, int H, int W, const vrgdg_adjust_desc* d) {

@@ -138,21 +138,27 @@ class ColorMatchToReference:
             raise ValueError("reference_image batch (%d) must be 1 or match images batch (%d)" % (n_ref, images.shape[0]))
         dev = compute_device(images)
         t = float(match_strength)
-        with torch.cuda.device(dev):
-            ref_sums = ops.lab_moments(upload(reference_image, dev).to(images.dtype))
+        ref_sums = None
+        if n_ref == 1:
+            with torch.cuda.device(dev):
+                ref_sums = ops.lab_moments(upload(reference_image, dev).to(images.dtype))
         d = nv.ChainDesc()
         d.colormatch_enabled, d.cm_t, d.cm_one_minus_t = 1, t, 1.0 - t
 
         def make_fn(card):
-            # the reference sums are made once and copied to each card; the scratch is the worker's own (two workers on one card
-            # must not share one)
-            sums = ref_sums.to(card)
+            # one reference: its sums are made once and copied to each card.  A reference clip (n_ref == B) stays where the caller
+            # keeps it; each chunk uploads only the reference frames of its own absolute indices and converts them on its card, so
+            # device memory follows the chunk, not the clip.  The scratch is the worker's own (two workers on one card must not share one)
+            sums = ref_sums.to(card) if n_ref == 1 else None
             state = {"scratch": None}
             def run(frames, first):
-                # one library call per chunk: statistics, parameters and the apply pass (which starts from the stored Lab f-planes
-                # for fp32 frames instead of repeating the forward transform)
-                rs = sums if n_ref == 1 else sums[first:first + frames.shape[0]]
-                out, state["scratch"] = ops.chain_cm_apply(frames, d, rs, scratch=state["scratch"])
+                # one library call per chunk: (the reference frames' statistics,) statistics, parameters and the apply pass (which
+                # starts from the stored Lab f-planes for fp32 frames instead of repeating the forward transform)
+                if n_ref == 1:
+                    out, state["scratch"] = ops.chain_cm_apply(frames, d, sums, scratch=state["scratch"])
+                    return out
+                refs = upload(reference_image[first:first + frames.shape[0]], card).to(frames.dtype)
+                out, state["scratch"] = ops.chain_cm_apply_refs(frames, d, refs, scratch=state["scratch"])
                 return out
             return run
         devs = devices_from_env() if images.device.type == "cpu" else None

@@ -269,6 +269,33 @@ def chain_cm_apply(images, desc, ref_sums, ext_noise=None, out=None, fast_math=F
     return out, scratch
 
 
+def chain_cm_apply_refs(images, desc, ref_frames, ext_noise=None, out=None, fast_math=False, recompute=False, group_frames=0, scratch=None,
+                        serial=False):
+    """chain_cm_apply against a reference clip in ONE library call (vrgdg_chain_cm_apply_refs): frame b is matched to ref_frames[b],
+    whose statistics the call makes group by group.  ref_frames: [B,Hr,Wr,3] in the images' dtype on their device, any Hr x Wr.
+    Bit-identical to chain_cm_apply(images, desc, lab_moments(ref_frames)).  Returns (out, scratch) as chain_cm_apply does."""
+    t = _frames(images)
+    r = _frames(ref_frames, "ref_frames")
+    B, H, W, _ = t.shape
+    if r.shape[0] != B or r.dtype != t.dtype or r.device != t.device:
+        raise ValueError("vrgdg_b200: ref_frames must hold %d frames of dtype %s on %s, got %d of %s on %s"
+                         % (B, t.dtype, t.device, r.shape[0], r.dtype, r.device))
+    out = torch.empty_like(t) if out is None else _check_out(out, t)
+    flags = _cm_flags(fast_math, recompute, serial)
+    lib = nv.load_library()
+    need = int(lib.vrgdg_chain_cm_scratch_bytes(B, H, W, nv.DTYPE_CODE[t.dtype], flags, int(group_frames)))
+    if scratch is None or scratch.numel() * scratch.element_size() < need or scratch.device != t.device:
+        scratch = torch.empty((max(need, 256),), dtype=torch.uint8, device=t.device)
+    ref_sums = torch.empty((B, 7), dtype=torch.float64, device=t.device)
+    n = _noise(ext_noise, t) if ext_noise is not None else None
+    with torch.cuda.device(t.device):
+        nv.check(lib.vrgdg_chain_cm_apply_refs(nv.ptr(t), nv.ptr(out), B, H, W, nv.DTYPE_CODE[t.dtype], ctypes.byref(desc), nv.ptr(r),
+                                               int(r.shape[1]), int(r.shape[2]), nv.ptr(ref_sums), nv.ptr(n), flags, nv.ptr(scratch),
+                                               ctypes.c_int64(scratch.numel() * scratch.element_size()), int(group_frames),
+                                               nv.stream_ptr(t.device)))
+    return out, scratch
+
+
 def chain_lab_moments(images, desc, ext_noise=None):
     """LAB sums [B,7] of stage 1 (grain) of `desc` applied to images; ext_noise: the N(0,1) tensor a chain_apply(ext_noise=...) will use."""
     t = _frames(images)

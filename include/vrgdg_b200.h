@@ -301,6 +301,27 @@ VRGDG_API int vrgdg_chain_cm_apply(const void* in, void* out, int B, int H, int 
                          const double* ref_sums, int n_ref, const void* ext_noise, int flags,
                          void* scratch, int64_t scratch_bytes, int group_frames, void* stream);
 
+/* vrgdg_chain_cm_apply against a reference CLIP: frame b is matched to reference frame b.  ref_frames [B][Hr][Wr][3] are in the
+ * frames' dtype, on the frames' device; Hr x Wr may differ from H x W (the statistics do not depend on the size).  For each group the
+ * call first runs vrgdg_lab_moments' statistics kernel (no grain, no f-planes) over the group's reference frames, then
+ * vrgdg_chain_cm_apply's statistics, parameters (n_ref = the group's size) and apply passes unchanged.  In the pipelined schedule
+ * the reference statistics of group g+1 run on the low-priority statistics stream ahead of that group's frame statistics, under the
+ * apply pass of group g; in the serial and recompute schedules they run just before the group's frame statistics.  The result is
+ * bit-identical to vrgdg_lab_moments over the whole reference clip followed by vrgdg_chain_cm_apply with n_ref = B: the sums are
+ * per frame and their reduction order is fixed, so neither the grouping nor the reference frame size changes a bit.
+ * ref_sums: a caller-owned [B][7] double buffer on the device, 8-byte aligned; it holds the reference frames' sums when the call
+ * completes.  scratch: vrgdg_chain_cm_scratch_bytes(B, H, W, dtype, flags, group_frames) bytes, as vrgdg_chain_cm_apply (the
+ * reference statistics share its partial sums).
+ * Pairing: frame b always takes reference b, whatever the chunk or group that carries it.  The reference's match_color broadcasts
+ * its [b,3,1,1] mini-batch statistics against the [B_ref,3,1,1] reference statistics, which pairs frame i with reference i only
+ * when one mini-batch spans the clip; this library pairs them at every batch size (as vrgdg_chain_cm_apply with n_ref = B does).
+ * Checked before any CUDA call, with the cases vrgdg_chain_cm_apply refuses: uint8 frames are VRGDG_E_UNSUPPORTED, Hr or Wr < 1
+ * VRGDG_E_INVALID, and for a non-empty batch a null ref_frames or ref_sums VRGDG_E_INVALID (a misaligned one VRGDG_E_ALIGN).  An
+ * empty batch with otherwise valid arguments is a successful no-op. */
+VRGDG_API int vrgdg_chain_cm_apply_refs(const void* in, void* out, int B, int H, int W, int dtype, const vrgdg_chain_desc* desc,
+                              const void* ref_frames, int Hr, int Wr, double* ref_sums, const void* ext_noise, int flags,
+                              void* scratch, int64_t scratch_bytes, int group_frames, void* stream);
+
 /* ---- "adjust" pass of the Builder UI ---------------------------------------------------------------------------
  * Replaces _apply_adjust_tensor (VRGDG_LUTVideoTools.py:307-391): clamp, temperature/tint offset, exposure, contrast,
  * saturation, highlight/shadow/white/black masks, clarity (k x k reflect-padded box, k = min(9, odd(H), odd(W))), sharpen
