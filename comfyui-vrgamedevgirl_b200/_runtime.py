@@ -1,4 +1,5 @@
 """Device policy and host<->device frame streaming shared by the node classes."""
+import math
 import os
 import threading
 
@@ -175,7 +176,17 @@ def bind_to_gpu_numa(device_index):
         return None
 
 
-def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, lane=0):
+def _result_shape(src, out_frame_shape):
+    """Shape of the streamed result: the source's, or [B, *out_frame_shape] for a fn whose frames change shape."""
+    return tuple(src.shape) if out_frame_shape is None else (int(src.shape[0]),) + tuple(int(d) for d in out_frame_shape)
+
+
+def _check_out(out, shape, dtype, out_device):
+    if tuple(out.shape) != tuple(shape) or out.dtype != dtype or out.device != out_device:
+        raise ValueError("vrgdg_b200: `out` must be a %s tensor of the result's shape %s on %s" % (dtype, list(shape), out_device))
+
+
+def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, lane=0, out_frame_shape=None):
     """Apply fn(cuda_frames, first_frame_index) -> cuda_frames over src [B,...] in chunks of `chunk` frames (0 / None = all).
 
     CUDA input: chunked as well (the reference bounds device memory with its batch_size widget the same way, nodes.py:49-62);
@@ -183,16 +194,22 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, la
     reusable staging buffers while chunk k computes and earlier results download; only the last download is waited for.
     Pinned source / result tensors make the copies truly asynchronous (the result is pinned when the source is).  `out`:
     optional preallocated result on out_device (reused across calls so that pinning cost is paid once).  `lane`: which pair of
-    the device's upload / download streams carries the copies (stream_frames_sharded gives each worker on a card its own)."""
+    the device's upload / download streams carries the copies (stream_frames_sharded gives each worker on a card its own).
+    `out_frame_shape`: the shape of one result frame when fn changes it (a resample); fn then returns [n, *out_frame_shape] in the
+    source dtype, pipeline chunks are sized on the larger of an input and a result frame, and fn is called for a host chunk only once
+    the result of the chunk `depth`+1 before it has downloaded, so results larger than their inputs cannot pile up on the device
+    while the download falls behind.  None: result frames have the source frames' shape."""
     B = int(src.shape[0])
     out_device = torch.device(out_device)
     chunk = B if chunk is None or int(chunk) <= 0 else min(int(chunk), max(B, 1))
+    out_shape = _result_shape(src, out_frame_shape)
+    out_bytes = math.prod(out_shape) * src.element_size()
     if src.device.type == "cuda":
         if chunk >= B:
             res = fn(src, 0)
             return res if res.device == out_device else res.to(out_device)
         to_host = out_device.type == "cpu"
-        res = torch.empty(src.shape, dtype=src.dtype, device=out_device, pin_memory=to_host and _pin_result(src, src.numel() * src.element_size()))
+        res = torch.empty(out_shape, dtype=src.dtype, device=out_device, pin_memory=to_host and _pin_result(src, out_bytes))
         for i in range(0, B, chunk):
             res[i:i + chunk].copy_(fn(src[i:i + chunk], i), non_blocking=to_host)
         if to_host:
@@ -200,13 +217,16 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, la
         return res
     dev = device if device is not None else compute_device()
     if B == 0:
+        if out_frame_shape is not None:
+            return torch.empty(out_shape, dtype=src.dtype, device=out_device)
         return torch.empty_like(src, device=out_device)
     src = src.contiguous()
     to_cpu = out_device.type == "cpu"
     # Host frames move in pipeline chunks of at most VRGDG_STREAM_CHUNK_BYTES (default 256 MiB, at least one frame): a chunk as large
     # as the batch would serialise upload, kernels and download.  Every caller's fn is independent of how the batch is cut (noise is
-    # keyed by the absolute frame index, statistics are per frame, temporal neighbours are fetched by index).
-    chunk = pipeline_chunk(chunk, src[0].numel() * src.element_size())
+    # keyed by the absolute frame index, statistics are per frame, temporal neighbours are fetched by index).  The cap holds for the
+    # larger of a source and a result frame, so that an upscale's result chunk stays within it too.
+    chunk = pipeline_chunk(chunk, max(src[0].numel() * src.element_size(), out_bytes // B))
     # A pageable source is staged through two pinned buffers by a multi-threaded host copy (torch's CPU copy_), so the DMA engine
     # reads pinned memory at PCIe speed while the next chunk is staged; the driver's own pageable path is a single-threaded bounce copy.
     stage = None
@@ -220,16 +240,17 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, la
         compute = torch.cuda.current_stream(dev)
         up, down = _side_streams(dev, lane)
         if out is None:
-            out = torch.empty(src.shape, dtype=src.dtype, pin_memory=_pin_result(src, src.numel() * src.element_size())) if to_cpu \
-                else torch.empty(src.shape, dtype=src.dtype, device=out_device)
-        elif out.shape != src.shape or out.dtype != src.dtype or out.device != out_device:
-            raise ValueError("vrgdg_b200: `out` must match the source frames in shape and dtype and live on %s" % out_device)
+            out = torch.empty(out_shape, dtype=src.dtype, pin_memory=_pin_result(src, out_bytes)) if to_cpu \
+                else torch.empty(out_shape, dtype=src.dtype, device=out_device)
+        else:
+            _check_out(out, out_shape, src.dtype, out_device)
         n_chunks = (B + chunk - 1) // chunk
         slots = [torch.empty((chunk,) + tuple(src.shape[1:]), dtype=src.dtype, device=dev) for _ in range(min(n_chunks, max(1, int(depth)) + 1))]
         for b in slots:
             b.record_stream(up)
         up.wait_stream(compute)                 # the staging buffers may recycle memory the compute stream is still using
         slot_free = [None] * len(slots)         # event: the kernels that read this slot have finished
+        downloaded = []                         # event per chunk: its result has reached `out` (kept only for out_frame_shape)
         for ci, i in enumerate(range(0, B, chunk)):
             s, n = ci % len(slots), min(chunk, B - i)
             host = src[i:i + n]
@@ -248,6 +269,8 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, la
             if stage is not None:
                 stage_free[ci % 2] = ev_up
             compute.wait_event(ev_up)
+            if out_frame_shape is not None and ci >= len(slots):
+                downloaded[ci - len(slots)].synchronize()   # its result block is free again before fn allocates this one's
             d_out = fn(slots[s][:n], i)
             ev_done = torch.cuda.Event()
             ev_done.record(compute)
@@ -256,6 +279,9 @@ def stream_frames(src, fn, chunk, out_device, device=None, out=None, depth=2, la
             with torch.cuda.stream(down):
                 d_out.record_stream(down)
                 out[i:i + n].copy_(d_out, non_blocking=True)
+                if out_frame_shape is not None:
+                    downloaded.append(torch.cuda.Event())
+                    downloaded[-1].record(down)
             del d_out
         ev_last = torch.cuda.Event()
         ev_last.record(down)
@@ -270,7 +296,7 @@ def shard_plan(n_frames, n_shards):
     return [shard_range(n_frames, k, n_shards) for k in range(n_shards)]
 
 
-def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None):
+def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None, out_frame_shape=None):
     """stream_frames over several CUDA devices from one process: host frames src [B,...] are cut into one contiguous shard per entry
     of `devices` (shard_plan), and each non-empty shard runs the stream_frames pipeline on its device in a host thread of its own,
     writing its slice of one shared result (pinned under stream_frames' rule).
@@ -281,19 +307,21 @@ def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None):
     workers get separate upload / download streams.  Kernels go to the calling thread's current stream of each device; a pageable
     source is staged through pinned buffers of each worker's own.  An exception in a worker is raised here after every worker has
     finished, and no thread outlives the call.  One device, a CUDA source or a CUDA out_device: one stream_frames call on one
-    device (CUDA batches are not sharded)."""
+    device (CUDA batches are not sharded).  `out_frame_shape`: as stream_frames'; every worker passes it on."""
     devices = [cuda_device(d) for d in devices]
     if not devices:
         raise ValueError("vrgdg_b200: stream_frames_sharded needs at least one CUDA device")
     out_device = torch.device(out_device)
+    shape_kw = {} if out_frame_shape is None else {"out_frame_shape": out_frame_shape}
     if len(devices) == 1 or src.device.type == "cuda" or out_device.type != "cpu":
         dev = src.device if src.device.type == "cuda" else devices[0]
-        return stream_frames(src, make_fn(dev), chunk, out_device, dev, out=out)
+        return stream_frames(src, make_fn(dev), chunk, out_device, dev, out=out, **shape_kw)
     src = src.contiguous()
+    out_shape = _result_shape(src, out_frame_shape)
     if out is None:
-        out = torch.empty(src.shape, dtype=src.dtype, pin_memory=_pin_result(src, src.numel() * src.element_size()))
-    elif out.shape != src.shape or out.dtype != src.dtype or out.device != out_device:
-        raise ValueError("vrgdg_b200: `out` must match the source frames in shape and dtype and live on %s" % out_device)
+        out = torch.empty(out_shape, dtype=src.dtype, pin_memory=_pin_result(src, math.prod(out_shape) * src.element_size()))
+    else:
+        _check_out(out, out_shape, src.dtype, out_device)
     jobs, lanes = [], {}
     for dev, (a, b) in zip(devices, shard_plan(int(src.shape[0]), len(devices))):
         if b > a:
@@ -304,7 +332,7 @@ def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None):
     def work(k, dev, lane, a, b, fn, stream):
         try:
             with torch.cuda.device(dev), torch.cuda.stream(stream):
-                stream_frames(src[a:b], lambda f, i: fn(f, a + i), chunk, out_device, dev, out=out[a:b], lane=lane)
+                stream_frames(src[a:b], lambda f, i: fn(f, a + i), chunk, out_device, dev, out=out[a:b], lane=lane, **shape_kw)
         except BaseException as e:               # re-raised in the calling thread
             errors[k] = e
 
@@ -322,10 +350,12 @@ def stream_frames_sharded(src, make_fn, chunk, out_device, devices, out=None):
     return out
 
 
-def run_frames(images, make_fn, chunk, out_device, device, devices):
+def run_frames(images, make_fn, chunk, out_device, device, devices, out_frame_shape=None):
     """The frame loop of every node.  A host batch with a host result is sharded over `devices` (the node's devices_from_env(),
     None = not sharded) by stream_frames_sharded; anything else is the single-device stream_frames(images, make_fn(device), ...).
-    make_fn(dev) -> fn(cuda_frames, absolute_first_frame) is called in the calling thread, once per non-empty shard."""
+    make_fn(dev) -> fn(cuda_frames, absolute_first_frame) is called in the calling thread, once per non-empty shard.
+    `out_frame_shape`: the shape of one result frame when fn changes it (stream_frames); None passes nothing on."""
+    shape_kw = {} if out_frame_shape is None else {"out_frame_shape": out_frame_shape}
     if devices is not None and images.device.type == "cpu" and torch.device(out_device).type == "cpu":
-        return stream_frames_sharded(images, make_fn, chunk, out_device, devices)
-    return stream_frames(images, make_fn(device), chunk, out_device, device)
+        return stream_frames_sharded(images, make_fn, chunk, out_device, devices, **shape_kw)
+    return stream_frames(images, make_fn(device), chunk, out_device, device, **shape_kw)

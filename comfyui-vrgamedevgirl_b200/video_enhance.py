@@ -39,15 +39,23 @@ def _output_size(resampled, offset, target_width, target_height, fit_mode):
 
 
 def _resize_batch(images, target_width, target_height, fit_mode, resize_method, _roi=None):
+    """The result has the input's device and dtype.  A CUDA batch is one vrgdg_resize launch.  A host batch streams through
+    run_frames like every frame node's IMAGE: VRGDG_STREAM_CHUNK_BYTES chunks (sized on the larger of an input and an output frame),
+    sharded over VRGDG_DEVICES, one launch per chunk with the same plan, so device and pinned host memory follow the chunk, not the
+    clip.  Every output frame depends only on its own input frame, so the result does not depend on the cut."""
     if images.ndim != 4 or images.shape[0] < 1:
         raise ValueError("Video Enhance requires a non-empty IMAGE batch.")
     dev = compute_device(images)
-    src = upload(images, dev)
-    x0, y0, sw, sh = _roi if _roi is not None else (0, 0, int(src.shape[2]), int(src.shape[1]))
+    x0, y0, sw, sh = _roi if _roi is not None else (0, 0, int(images.shape[2]), int(images.shape[1]))
     resampled, offset = _resize_plan(sw, sh, target_width, target_height, fit_mode)
     ow, oh = _output_size(resampled, offset, target_width, target_height, fit_mode)
-    out = ops.resize(src, oh, ow, _interpolation(resize_method), roi=(x0, y0, sw, sh), resampled=resampled, offset=offset)
-    return out.to(images.device)
+    mode = _interpolation(resize_method)
+
+    def make_fn(card):
+        return lambda frames, first: ops.resize(frames, oh, ow, mode, roi=(x0, y0, sw, sh), resampled=resampled, offset=offset)
+
+    devs = devices_from_env() if images.device.type == "cpu" else None
+    return run_frames(images, make_fn, 0, images.device, dev, devs, out_frame_shape=(oh, ow, 3))
 
 
 def _restore_roi(work_w, work_h, source_width, source_height, fit_mode):
