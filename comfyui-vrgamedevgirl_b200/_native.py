@@ -130,6 +130,8 @@ SIGNATURES = {
     "vrgdg_hist_counts": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "vrgdg_histmatch_tables": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "vrgdg_histmatch_apply": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _f, _f, _vp]),
+    "vrgdg_histmatch_refs_scratch_bytes": (_i64, [_i]),
+    "vrgdg_histmatch_apply_refs": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _f, _f, _vp, _i64, _vp]),
     "vrgdg_temporal_sharpen": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
     "vrgdg_lanczos4_tables": (_i, [_i, _i, _vp, _vp]),
     "vrgdg_lanczos4_scratch_bytes": (_i64, [_i, _i, _i]),

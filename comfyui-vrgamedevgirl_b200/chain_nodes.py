@@ -161,9 +161,12 @@ class VRGDG_B200_EnhanceFrames:
 
 
 class VRGDG_B200_HistogramColorMatch:
-    """Histogram / CDF colour transfer to one reference image: per-channel 256-bin histograms, monotone CDF mapping (the colour-match
+    """Histogram / CDF colour transfer to a reference image: per-channel 256-bin histograms, monotone CDF mapping (the colour-match
     mode BASELINE.json describes).  An extension of this package: the reference's ColorMatchToReference is the LAB mean/std transfer
-    and stays that; the arithmetic of this mode is specified in include/vrgdg_b200.h (vrgdg_hist_counts ...)."""
+    and stays that; the arithmetic of this mode is specified in include/vrgdg_b200.h (vrgdg_hist_counts ...).  reference_image holds
+    one frame or one per frame, as ColorMatchToReference's does: with B frames, frame i is matched to reference frame i at every
+    batch_size, and each chunk uploads only its own reference frames (vrgdg_histmatch_apply_refs), so the clip never has to fit
+    on the card."""
 
     @classmethod
     def INPUT_TYPES(cls):
@@ -185,19 +188,31 @@ class VRGDG_B200_HistogramColorMatch:
         from . import ops
         images = _as_frames(images)
         ref = _as_frames(reference_image, "reference_image")
-        if int(ref.shape[0]) != 1:
-            raise ValueError("VRGDG_B200_HistogramColorMatch: reference_image must hold exactly one frame")
+        n_ref = int(ref.shape[0])
+        if n_ref != 1 and n_ref != int(images.shape[0]):
+            raise ValueError("reference_image batch (%d) must be 1 or match images batch (%d)" % (n_ref, images.shape[0]))
         dev = compute_device(images)
         t = float(match_strength)
-        with torch.cuda.device(dev):
-            ref_counts = ops.hist_counts(upload(ref, dev).to(images.dtype))
+        ref_counts = None
+        if n_ref == 1:
+            with torch.cuda.device(dev):
+                ref_counts = ops.hist_counts(upload(ref, dev).to(images.dtype))
 
         def make_fn(card):
-            counts = ref_counts.to(card)         # made once, copied to each card
-            def run(frames, first):
-                tables = ops.histmatch_tables(ops.hist_counts(frames), counts)
-                return ops.histmatch_apply(frames, tables, t, 1.0 - t)
-            return run
+            if n_ref == 1:
+                counts = ref_counts.to(card)         # made once, copied to each card
+                def run(frames, first):
+                    tables = ops.histmatch_tables(ops.hist_counts(frames), counts)
+                    return ops.histmatch_apply(frames, tables, t, 1.0 - t)
+                return run
+            # a reference clip stays where the caller keeps it; each chunk uploads the reference frames of its own absolute indices
+            # and converts them on its card.  The scratch is the worker's own (two workers on one card must not share one)
+            state = {"scratch": None}
+            def run_clip(frames, first):
+                refs = upload(ref[first:first + frames.shape[0]], card).to(frames.dtype)
+                out, state["scratch"] = ops.histmatch_apply_refs(frames, refs, t, 1.0 - t, scratch=state["scratch"])
+                return out
+            return run_clip
         devs = devices_from_env() if images.device.type == "cpu" else None
         return (run_frames(images, make_fn, batch_size, result_device(images), dev, devs),)
 

@@ -1092,6 +1092,62 @@ int vrgdg_histmatch_apply(const void* in, void* out, int B, int H, int W, int dt
   return VRGDG_OK;
 }
 
+/* scratch of vrgdg_histmatch_apply_refs, per frame: the edge tables (float2, first, so 8-byte aligned), the frame counts and the
+ * reference counts (uint32) */
+int64_t vrgdg_histmatch_refs_scratch_bytes(int B) {
+  if (B <= 0) return 0;
+  return (int64_t)B * 3 * HIST_BINS * (int64_t)(sizeof(float2) + 2 * sizeof(uint32_t));
+}
+
+int vrgdg_histmatch_apply_refs(const void* in, void* out, int B, int H, int W, int dtype, const void* ref_frames, int Hr, int Wr,
+                               float t, float one_minus_t, void* scratch, int64_t scratch_bytes, void* stream) {
+  const char* who = "vrgdg_histmatch_apply_refs";
+  if (dtype == VRGDG_U8BGR) return fail(VRGDG_E_UNSUPPORTED, "%s: uint8 frames are not supported (reference clips are float IMAGE tensors)", who);
+  if (Hr < 1 || Wr < 1) return fail(VRGDG_E_INVALID, "%s: bad reference frame size %d x %d", who, Hr, Wr);
+  if ((int64_t)Hr * Wr >= (int64_t)1 << 31)
+    return fail(VRGDG_E_UNSUPPORTED, "%s: reference frame of %d x %d pixels exceeds 2^31 (32-bit counters)", who, Hr, Wr);
+  int rc = check_frames(in, out, B, H, W, dtype, who);
+  if (rc) return rc;
+  if ((int64_t)B * H * W == 0) return VRGDG_OK;
+  if (!ref_frames) return fail(VRGDG_E_INVALID, "%s: null ref_frames", who);
+  const size_t es = elem_size(dtype);
+  if (reinterpret_cast<uintptr_t>(ref_frames) % es) return fail(VRGDG_E_ALIGN, "%s: ref_frames not aligned to its element size", who);
+  if (!scratch) return fail(VRGDG_E_INVALID, "%s: null scratch", who);
+  if (reinterpret_cast<uintptr_t>(scratch) & 255u) return fail(VRGDG_E_ALIGN, "%s: scratch must be 256-byte aligned", who);
+  const int64_t need = vrgdg_histmatch_refs_scratch_bytes(B);
+  if (scratch_bytes < need) return fail(VRGDG_E_INVALID, "%s: scratch too small (%lld < %lld)", who, (long long)scratch_bytes, (long long)need);
+  LaunchCtx ctx;
+  if ((rc = get_ctx(stream, ctx))) return rc;
+  const int64_t per = (int64_t)3 * HIST_BINS;
+  float2* tables = reinterpret_cast<float2*>(scratch);
+  uint32_t* fcounts = reinterpret_cast<uint32_t*>(tables + (int64_t)B * per);
+  uint32_t* rcounts = fcounts + (int64_t)B * per;
+  // k_hist_counts takes one frame per grid row (gridDim.y <= 65535): count larger batches in slices of frames
+  auto counts = [&](const void* frames, int h, int w, uint32_t* dst) -> cudaError_t {
+    constexpr int SLICE = 65535;
+    for (int f0 = 0; f0 < B; f0 += SLICE) {
+      const int n = (B - f0 < SLICE) ? B - f0 : SLICE;
+      const void* src = reinterpret_cast<const char*>(frames) + (size_t)f0 * h * w * 3 * es;
+#define HC(T) launch_hist_counts<T>(src, n, h, w, 0, h, dst + (int64_t)f0 * per, ctx)
+      const cudaError_t e = DISPATCH_DTYPE(dtype, HC);
+#undef HC
+      if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+  };
+  cudaError_t e = counts(in, H, W, fcounts);
+  if (e == cudaSuccess) e = counts(ref_frames, Hr, Wr, rcounts);
+  if (e != cudaSuccess) return fail_cuda(e, "vrgdg_histmatch_apply_refs (counts)");
+  k_hist_tables<<<(unsigned)((int64_t)B * 3), 256, 0, ctx.stream>>>(fcounts, rcounts, B, tables);
+  count_launch();
+  if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "vrgdg_histmatch_apply_refs (tables)");
+#define HA(T) launch_histmatch_apply<T>(in, out, B, (int64_t)H * W, tables, t, one_minus_t, ctx)
+  e = DISPATCH_DTYPE(dtype, HA);
+#undef HA
+  if (e != cudaSuccess) return fail_cuda(e, "vrgdg_histmatch_apply_refs (apply)");
+  return VRGDG_OK;
+}
+
 int vrgdg_temporal_sharpen(const void* in, void* out, int B, int H, int W, int dtype, float strength, const void* prev_frame,
                            const void* next_frame, void* stream) {
   int rc = check_frames(in, out, B, H, W, dtype, "vrgdg_temporal_sharpen");

@@ -437,6 +437,29 @@ def histmatch_apply(images, tables, t_strength, one_minus_t):
     return out
 
 
+def histmatch_apply_refs(images, ref_frames, t_strength, one_minus_t, scratch=None):
+    """Histogram colour match against a reference clip in ONE library call (vrgdg_histmatch_apply_refs): frame b is matched to
+    ref_frames[b].  ref_frames: [B,Hr,Wr,3] in the images' dtype on their device, any Hr x Wr.  torch.equal to
+    histmatch_apply(images, histmatch_tables(hist_counts(images), hist_counts(ref_frames)), t_strength, one_minus_t).
+    Returns (out, scratch); hand the scratch back to the next call to reuse it."""
+    t = _frames(images)
+    r = _frames(ref_frames, "ref_frames")
+    B, H, W, _ = t.shape
+    if r.shape[0] != B or r.dtype != t.dtype or r.device != t.device:
+        raise ValueError("vrgdg_b200: ref_frames must hold %d frames of dtype %s on %s, got %d of %s on %s"
+                         % (B, t.dtype, t.device, r.shape[0], r.dtype, r.device))
+    out = torch.empty_like(t)
+    lib = nv.load_library()
+    need = int(lib.vrgdg_histmatch_refs_scratch_bytes(B))
+    if scratch is None or scratch.numel() * scratch.element_size() < need or scratch.device != t.device:
+        scratch = torch.empty((max(need, 256),), dtype=torch.uint8, device=t.device)
+    with torch.cuda.device(t.device):
+        nv.check(lib.vrgdg_histmatch_apply_refs(nv.ptr(t), nv.ptr(out), B, H, W, nv.DTYPE_CODE[t.dtype], nv.ptr(r), int(r.shape[1]),
+                                                int(r.shape[2]), _f32(t_strength), _f32(one_minus_t), nv.ptr(scratch),
+                                                ctypes.c_int64(scratch.numel() * scratch.element_size()), nv.stream_ptr(t.device)))
+    return out, scratch
+
+
 def temporal_sharpen(images, strength, prev_frame=None, next_frame=None):
     """3-frame temporal unsharp over a clip [T,H,W,3] (configs[4]; labelled extension, see vrgdg_temporal_sharpen).  prev_frame /
     next_frame: [H,W,3] (or [1,H,W,3]) neighbours of the first / last frame when the clip is a shard of a longer one."""

@@ -387,6 +387,26 @@ VRGDG_API int vrgdg_histmatch_tables(const uint32_t* frame_counts, int B, const 
 VRGDG_API int vrgdg_histmatch_apply(const void* in, void* out, int B, int H, int W, int dtype, const float* tables,
                           float t, float one_minus_t, void* stream);
 
+/* The histogram colour match against a reference CLIP in one call: frame b is matched to reference frame b.  ref_frames
+ * [B][Hr][Wr][3] are in the frames' dtype, on the frames' device; Hr x Wr may differ from H x W (the counts do not depend on the size).
+ * The call enqueues on `stream`, with no host synchronisation: vrgdg_hist_counts' kernel over the B frames, the same kernel over the
+ * B reference frames at Hr x Wr, vrgdg_histmatch_tables' kernel with n_ref = B and vrgdg_histmatch_apply's kernel.  The result is
+ * bit-identical to those four calls made one by one: the counts are exact integers and the tables are per frame.
+ * Pairing: frame b always takes reference b, whatever the chunk or call that carries it, so a clip cut into chunks (reference frames
+ * sliced by the same absolute indices) gives what one call over the clip gives, and a clip of B copies of one frame gives
+ * vrgdg_histmatch_tables with n_ref = 1.
+ * scratch: vrgdg_histmatch_refs_scratch_bytes(B) bytes of device memory (the counts of both and the tables, about 12 KB per frame),
+ * 256-byte aligned, owned by the caller, contents undefined afterwards; reusable by the next call on the same stream.  `out` may
+ * be `in`: every count is taken before the apply pass writes.
+ * Checked before any CUDA call: uint8 frames are VRGDG_E_UNSUPPORTED (reference clips are float IMAGE tensors), Hr or Wr < 1
+ * VRGDG_E_INVALID and Hr x Wr >= 2^31 VRGDG_E_UNSUPPORTED (32-bit counters), then the frames as vrgdg_histmatch_apply checks them;
+ * for a non-empty batch a null ref_frames or scratch is VRGDG_E_INVALID, a misaligned one VRGDG_E_ALIGN and a scratch smaller
+ * than vrgdg_histmatch_refs_scratch_bytes(B) VRGDG_E_INVALID.  An empty batch with otherwise valid arguments is a successful no-op.
+ * vrgdg_histmatch_refs_scratch_bytes is 0 for B <= 0 and grows with B. */
+VRGDG_API int64_t vrgdg_histmatch_refs_scratch_bytes(int B);
+VRGDG_API int vrgdg_histmatch_apply_refs(const void* in, void* out, int B, int H, int W, int dtype, const void* ref_frames,
+                               int Hr, int Wr, float t, float one_minus_t, void* scratch, int64_t scratch_bytes, void* stream);
+
 /* ---- temporal 3-frame unsharp (BASELINE.json configs[4]) — LABELLED EXTENSION, no reference counterpart --------------------
  * The reference has no temporal operator (VRGDG_VideoEnhanceNodes.py holds no sharpen / blur / stencil; SURVEY D4), so the
  * specification is this library's:  out[t] = clamp(x[t] + s * (x[t] - (x[t-1] + x[t] + x[t+1]) / 3), 0, 1), fp32, one rounding
